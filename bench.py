@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — NRSC-5 FM receive-chain throughput on B200 (see DESIGN.md §measurement).
+"""bench.py — NRSC-5 FM receive-chain throughput on H100 (see DESIGN.md §measurement).
 
 Metric (BASELINE.json): cu8 I/Q Msamples/s (complex samples; / 1.488375 = x real
 time) of the whole hot path, at N GPUs, streams sharded per GPU, weak scaling.
@@ -18,7 +18,8 @@ FM MP1 channels per GPU (config 5's per-GPU shard: 128 channels), each
           reference built into oracle/_ref/libnrsc5_ref.so; FFTW replaced by
           oracle/shim/fftshim.c) on the host cores, same captures.
 
-One JSON line on stdout (rank 0).
+One JSON line on stdout (rank 0).  --dump-outputs DIR also writes the records the
+last timed device-resident step decoded, as .npy arrays (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -41,6 +42,12 @@ DEMOD_BYTES_PER_BLOCK = 276480 + 32 * 534 * 8      # cu8 in + 534 complex bins x
 FUSED_BYTES_PER_BLOCK = 276480 + 23040              # SURVEY §8(d): cu8 in + int8 soft bits out
 P1_BYTES_PER_FRAME = 368640 + 18272 + 160           # SURVEY §8(d)
 SYNC_BYTES_PER_BLOCK = 32 * 534 * 8 + 23040
+# H100 SXM data-sheet peaks (700 W card) for the roofline fractions, and its maximum SM clock (what the engine's
+# per-phase cycle counters are turned into microseconds with when no clock was sampled during the run)
+H100_HBM_GBS = 3350.0
+H100_INT8_TOPS = 1979.0
+H100_MAX_SM_MHZ = 1980.0
+DUMP_BUDGET_BYTES = 64 << 20
 
 
 def parse_args():
@@ -69,6 +76,7 @@ def parse_args():
     ap.add_argument("--mp3-frames", type=int, default=6)
     ap.add_argument("--am-streams", type=int, default=256)
     ap.add_argument("--am-frames", type=int, default=12)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's decoded records to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -151,7 +159,7 @@ def l2_leg(args):
     pk = [ev for r in l2 for t, ev in r["events"] if t == eng.EV_PACKET]
     assert len(l2) >= 2 and len(pk) >= 30 * (len(l2) - 1), (len(l2), len(pk))
     assert all(p["flags"] == 0 for p in pk) and not any(r["flags"] for r in l2)
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     ms_off = timed(False, steps)
     ms_on = timed(True, steps)
     e.set_profiling(True)
@@ -208,7 +216,7 @@ def mp3_leg(args):
           for rr in recs]
     assert nf[0][0] >= F - 1 and nf[0][1] >= 8 * (F - 2) - 2, nf[0]         # P3 output starts after two frames of interleaver fill
     first = [record_digest(r) for r in recs]
-    steps = max(2, min(args.steps, 3))
+    steps = args.steps
     tot = sum(step()[0] for _ in range(steps))
     res = 0.0
     for _ in range(steps):
@@ -263,7 +271,7 @@ def am_leg(args, engine_factory=None):
     assert len(p1) >= 8 * (F - 8), f"{len(p1)} AM P1 frames decoded from {F} transmitted L1 frames"
     gate = parity_gate(views, recs, am=True, what="am_config4")   # every channel: P1 / P3 / PIDS PDUs in order == oracle
     first = [record_digest(r) for r in recs]
-    steps = max(2, min(args.steps, 3))
+    steps = args.steps
     tot = proc = 0.0
     for _ in range(steps):
         a, b, _ = step()
@@ -271,18 +279,22 @@ def am_leg(args, engine_factory=None):
         proc += b
     # the same samples again, already resident in HBM: rewind (receiver state starts over) + process
     res = 0.0
+    sampler = ClockSampler(0)
+    sampler.start()
+    sampler.mark_begin()
     for _ in range(steps):
         e.rewind()
         t0 = time.perf_counter()
         e.process()
         res += time.perf_counter() - t0
+    clk_mhz, clk_src = sm_clock(sampler.stop())
     again = e.drain_all()
     assert [record_digest(r) for r in again] == first, "rewind -> process gave other records than reset -> push -> process"
     samples = S * (n // 2)
     try:
         pc = e.am_phase_cycles()                          # of the last rewind -> process
         nblk = max(1, int(e.stats().blocks))
-        am_phases = {k: round(v / nblk / 1965.0, 2) for k, v in pc.items() if k != "traceback_repair_rounds"}    # us per stream-block at 1965 MHz
+        am_phases = {k: round(v / nblk / clk_mhz, 2) for k, v in pc.items() if k != "traceback_repair_rounds"}    # us per stream-block
         am_phases["traceback_repair_rounds_per_block"] = round(pc.get("traceback_repair_rounds", 0) / nblk, 4)   # (a count, not a time)
     except Exception:                                     # noqa: BLE001
         am_phases = None
@@ -310,7 +322,7 @@ def am_leg(args, engine_factory=None):
                         "note": "latency-bound by construction: per stream the NCO phase chain (17 280 dependent complex multiplications "
                                 "per block, one warp) and the K=9 recursion (a verified chunk per warp, three trellis steps per metric "
                                 "exchange) are dependent chains; 256 streams put at most two CTAs on an SM", "blocks_total": blocks},
-           "cpu_baseline": cpu, "phases_us_per_stream_block_at_1965MHz": am_phases,
+           "cpu_baseline": cpu, "phases_us_per_stream_block": am_phases, "sm_clock_mhz": clk_mhz, "sm_clock_source": clk_src,
            "x_realtime": samples * steps / res / 46511.71875, "ms_per_step": 1e3 * res / steps,
            "e2e": {"value": samples * steps / tot / 1e6, "ms_per_step": 1e3 * tot / steps, "x_realtime": samples * steps / tot / 46511.71875,
                    "process_ms_per_step": 1e3 * proc / steps, "h2d_bytes_per_step": int(S * n * 2),
@@ -374,7 +386,7 @@ def dropin_leg(args):
 
 
 def chan_leg(args):
-    """SURVEY 8 f3: the wideband channeliser (csrc/channelizer.cu, tcgen05.mma.kind::i8).  One cu8 capture at 23.814 MS/s
+    """SURVEY 8 f3: the wideband channeliser (csrc/channelizer.cu, wgmma u8 x s8).  One cu8 capture at 23.814 MS/s
     resident in HBM -> 100 FM channels (the whole 88-108 MHz raster) at 744 187.5 S/s cs16, device to device.  Gate: a
     slice of the output equals the numpy restatement bit for bit.  Prints one JSON object."""
     import torch
@@ -407,7 +419,7 @@ def chan_leg(args):
         for _ in range(3):
             run()
         torch.cuda.synchronize()
-        steps = max(5, min(args.steps, 20))
+        steps = args.steps
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(stream)
         for _ in range(steps):
@@ -419,29 +431,55 @@ def chan_leg(args):
     groups = (len(offs) + 31) // 32
     macs = nout * groups * 128 * 512                           # int8 multiply-accumulates issued (rows of B incl. padding channels)
     useful = nout * len(offs) * 4 * 512
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    bf16 = float(peaks.get("bf16_tflops", 1660.8))
-    peak_i8 = 2 * bf16                                          # int8 runs at twice the bf16 rate; no int8 GEMM measurement in MEASURED_PEAKS.json
+    peak_i8 = H100_INT8_TOPS
     hbm, hbm_src = measured_peak()
     traffic = nbytes + len(offs) * nout * 4
-    dram = None
-    try:                                                   # DRAM bytes of one launch from the ncu capture of this very leg
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json"))).get("k_channelize")
-        dram = tj and (tj["dram_read_bytes"] + tj["dram_write_bytes"])
-    except Exception:                                      # noqa: BLE001
-        pass
     out_j = {"value": samples / (ms * 1e-3) / 1e6, "unit": "Msamples/s (wideband cu8 complex, 23.814 MS/s)", "ms_per_step": ms,
              "x_realtime": samples / (ms * 1e-3) / 23814000.0, "channels": len(offs), "outputs_per_channel": int(nout), "steps": steps,
              "channel_msamples_per_s": len(offs) * nout / (ms * 1e-3) / 1e6,
-             "roofline": {"bound": "tensor", "kernel": "k_channelize (tcgen05.mma.kind::i8, M128 N128 K512 per tile)",
+             "roofline": {"bound": "tensor", "kernel": "k_channelize (wgmma u8 x s8, M64 N128 K512 per tile)",
                           "achieved": 2 * macs / (ms * 1e-3) / 1e12, "useful": 2 * useful / (ms * 1e-3) / 1e12, "peak": peak_i8, "unit": "TOP/s",
                           "frac": 2 * macs / (ms * 1e-3) / 1e12 / peak_i8,
-                          "peak_source": "2 x MEASURED_PEAKS.json bf16_tflops (int8 tensor rate; no int8 measurement in that file)",
-                          "hbm_gbs": traffic / (ms * 1e-3) / 1e9, "hbm_frac": traffic / (ms * 1e-3) / 1e9 / hbm, "algorithmic_bytes": traffic,
-                          "traffic": dram, "traffic_source": "profiles/r2_ncu_summary.md (ncu --set full, one launch of this leg)"},
+                          "peak_source": "H100 SXM data sheet, dense INT8 at 700 W",
+                          "hbm_gbs": traffic / (ms * 1e-3) / 1e9, "hbm_frac": traffic / (ms * 1e-3) / 1e9 / hbm, "algorithmic_bytes": traffic},
              "parity_gate": {"ok": True, "what": "first 1493 and last 64 output samples of all 100 channels == oracle/chan_oracle.py"},
              "workload": "one 2^27-byte cu8 capture (uniform random bytes) resident in HBM -> 100 channels x %d cs16 samples, device to device" % nout}
     print(json.dumps(out_j), flush=True)
+
+
+def dump_outputs(path: str, recs_per_stream):
+    """Writes what a caller of the timed path receives, every stream's decoded records, as float arrays:
+      frame_pdus.npy  float32 [N, 18272]  bytes of every L1 PDU (packed bits, zero-padded), in stream and decode order
+      frame_meta.npy  float64 [N, 3]      (stream, logical channel, bits) of each of those PDUs
+      pids_pdus.npy   float32 [M, 10]     bytes of every PIDS PDU;  pids_meta.npy float64 [M] its stream
+      sync.npy        float64 [K, 3]      (stream, frequency offset in Hz, PSMI) of every sync event
+    Beyond DUMP_BUDGET_BYTES in all, the L1 PDU rows are a fixed, seeded sample (sorted, so still in order)."""
+    from nrsc5_b200 import engine as eng
+    os.makedirs(path, exist_ok=True)
+    frames, fmeta, pids, pmeta, sync = [], [], [], [], []
+    for s, recs in enumerate(recs_per_stream):
+        for t, r in recs:
+            if t == eng.REC_FRAME:
+                frames.append(r["bits"])
+                fmeta.append((s, r["lc"], r["nbits"]))
+            elif t == eng.REC_PIDS:
+                pids.append(r["bits"])
+                pmeta.append(s)
+            elif t == eng.REC_SYNC:
+                sync.append((s, r["freq_offset"], r["psmi"]))
+    width = max([len(b) for b in frames] + [18272])
+    keep = np.arange(len(frames))
+    budget = DUMP_BUDGET_BYTES - (8 << 20)                     # (what PIDS and sync events take is far below 8 MB)
+    if len(frames) * width * 4 > budget:
+        keep = np.sort(np.random.default_rng(0).choice(len(frames), budget // (width * 4), replace=False))
+    fr = np.zeros((len(keep), width), dtype=np.float32)
+    for i, k in enumerate(keep):
+        fr[i, :len(frames[k])] = np.frombuffer(frames[k], dtype=np.uint8)
+    np.save(os.path.join(path, "frame_pdus.npy"), fr)
+    np.save(os.path.join(path, "frame_meta.npy"), np.array(fmeta, dtype=np.float64).reshape(-1, 3)[keep])
+    np.save(os.path.join(path, "pids_pdus.npy"), np.array([np.frombuffer(b, dtype=np.uint8) for b in pids], dtype=np.float32).reshape(-1, 10))
+    np.save(os.path.join(path, "pids_meta.npy"), np.array(pmeta, dtype=np.float64))
+    np.save(os.path.join(path, "sync.npy"), np.array(sync, dtype=np.float64).reshape(-1, 3))
 
 
 def stream_views(caps, nstreams: int, rank: int):
@@ -513,8 +551,8 @@ def parity_gate(views, recs_per_stream, am=False, what=""):
 
 
 class ClockSampler:
-    """Samples SM clocks / throttle reasons with one streaming `nvidia-smi -lms` process (the recipe's
-    clocks line in B200_PROFILING.md); only the samples taken between mark_begin() and stop() count."""
+    """Samples SM clocks / throttle reasons with one streaming `nvidia-smi -lms` process; only the samples taken
+    between mark_begin() and stop() count."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -572,11 +610,16 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+def sm_clock(clocks):
+    """The SM clock (MHz) to turn the engine's cycle counters into microseconds: the median ClockSampler saw in the
+    timed window, or the H100's maximum when it saw none."""
+    if clocks and clocks.get("sm_mhz"):
+        return clocks["sm_mhz"], "median SM clock sampled during the timed steps"
+    return H100_MAX_SM_MHZ, "no clock samples: the H100 SXM maximum SM clock"
+
+
 def measured_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return H100_HBM_GBS, "H100 SXM data sheet (HBM3)"
 
 
 def cpu_reference_numbers(bufs, nbytes, reps, am=False):
@@ -652,7 +695,7 @@ def workload_config(args, nbytes):
                         f"(BASELINE config 5 shard), {args.frames} L1 frames + 2 blocks each, full chain to L1 PDUs",
             "streams_per_gpu": args.streams, "frames_per_stream": args.frames, "bytes_per_stream": int(nbytes),
             "distinct_captures": args.distinct,
-            "l2": "per-GPU input (streams x bytes_per_stream) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "per-GPU input (streams x bytes_per_stream) exceeds the 50 MB L2; no explicit flush"}
 
 
 def main():
@@ -789,6 +832,10 @@ def main():
 
     # ---- value: device-resident ----
     ms, launches, clocks, _ = timed(step_resident, args.steps, max(args.warmup, 3))
+    if args.dump_outputs and rank == 0:
+        last = e.drain_all()                      # the records of the last timed step (every step starts with a rewind)
+        assert [record_digest(r) for r in last] == resident_digests, "the timed steps decoded other records than the gated step"
+        dump_outputs(args.dump_outputs, last)
     total_samples = samples_per_step * world * args.steps
     value = total_samples / (ms * 1e-3) / 1e6
 
@@ -799,7 +846,7 @@ def main():
     kt = e.kernel_times()
     e.set_profiling(False)
     # where the front-end kernel's SM time goes: average microseconds per stream-block and phase
-    clk_mhz = 1965.0
+    clk_mhz, clk_src = sm_clock(clocks)
     phases = {k: {"us_per_call": (c / n / clk_mhz) if n else 0.0, "calls": n} for k, (c, n) in e.phase_cycles().items()}
     st = e.stats()
     peak, peak_src = measured_peak()
@@ -820,23 +867,12 @@ def main():
         gbs = alg[k] / (v["ms"] * 1e-3) / 1e9 if v["ms"] > 0 else 0.0
         kinfo[k] = {"ms_per_step": v["ms"], "launches": v["launches"], "alg_bytes_per_step": alg[k], "achieved_gbs": gbs}
     dom = max(("front", "p1"), key=lambda k: kt[k]["ms"])
-    # DRAM traffic of the dominant kernel from the committed ncu --set full capture, scaled to this run's
-    # average launch (bytes per stream-block x stream-blocks per launch)
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if not os.path.exists(tp):
-        tp = os.path.join(ROOT, "profiles", "r1_traffic.json")
-    if dom == "front" and os.path.exists(tp):
-        tj = json.load(open(tp))
-        per_block = (tj["k_stream"]["dram_read_bytes"] + tj["k_stream"]["dram_write_bytes"]) / tj["k_stream"]["stream_blocks"]
-        traffic = per_block * blocks_per_step / max(1, kt[dom]["launches"])
-        traffic_src = tj["source"]
     roofline = {"bound": "hbm", "kernel": "k_stream (stream-resident front end: prep+halfband+NCO+FFT+sync+demap)" if dom == "front" else "P1 decode group",
                 "achieved": kinfo[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                "frac": kinfo[dom]["achieved_gbs"] / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "frac": kinfo[dom]["achieved_gbs"] / peak, "peak_source": peak_src,
                 "alg_bytes_per_launch": alg[dom] / max(1, kt[dom]["launches"]),
                 "chain_frac_of_hbm": (2.34 * value * 1e6 / world) / (peak * 1e9),
-                "kernels": kinfo, "front_phases_at_1965MHz": phases,
+                "kernels": kinfo, "front_phases_us": phases, "sm_clock_mhz": clk_mhz, "sm_clock_source": clk_src,
                 "p1_frames_per_step": frames_per_step, "p1_fast_path_fallbacks": p1_fallbacks}
 
     # ---- e2e ----

@@ -1,4 +1,4 @@
-/* nrsc5_b200 — C ABI of the B200-native NRSC-5 FM physical-layer receive
+/* nrsc5_b200 — C ABI of the H100-native NRSC-5 FM physical-layer receive
  * engine (libnrsc5_b200.so).  Plain pointers and sizes only.
  *
  * What each entry point replaces in the reference (theori-io/nrsc5 @ a5c0972):
@@ -259,7 +259,7 @@ int nrsc5b_fft2048(int device, const float *in, float *out, int nffts);
  *     acc = sum_{u<256} W_k[u] * (x[32 n + u] - (127 + 127j));   v = (acc + 2^12) >> 13;
  *     y[k][n] = saturate16((v * conj(P[(1600 m_k n) mod 11907]) + 2^14) >> 15)
  * with the 16-bit taps W_k and the phasor table P as returned by nrsc5b_chan_tables.  Runs on the tensor cores
- * (tcgen05.mma.kind::i8, TMA-fed, accumulators in TMEM). */
+ * (wgmma u8 x s8, TMA-fed, accumulators in registers). */
 typedef struct nrsc5b_channelizer nrsc5b_channelizer_t;
 int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch);
 void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c);

@@ -1,4 +1,4 @@
-"""Builds libnrsc5_b200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.
+"""Builds libnrsc5_b200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.
 
 No torch extension machinery: the product boundary is a plain C-ABI shared
 library (include/nrsc5_b200.h) that ctypes, cgo or the reference's own C host
@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libnrsc5_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = (["-DNB_DEBUG"] if os.environ.get("NB_DEBUG") else []) + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 # (source, extra flags).  engine.cu keeps the reference's float operation order in the acquisition /

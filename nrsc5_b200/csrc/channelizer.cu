@@ -3,8 +3,8 @@
 // no such stage (its ingest is one narrowband device per handle, reference src/nrsc5.c:130-207, src/rtltcp.c); this is
 // the step in front of input_push_cs16 (src/input.c:119-124) that makes "many channels per GPU" a physical workload.
 //
-// It is the one dense contraction of the whole system, and the one kernel here that runs on the 5th-generation tensor
-// cores:  for channel k and output sample n
+// It is the one dense contraction of the whole system, and the one kernel here that runs on the tensor cores:  for
+// channel k and output sample n
 //
 //     acc[k][n] = sum_{u < 256} W_k[u] * (x[32 n + u] - (127 + 127j))        W_k[u] = round(2^19 h[255-u] e^{-j 2 pi 50 m_k u / 11907})
 //     y[k][n]   = sat16( ((acc + 2^12) >> 13) * conj(P[(1600 m_k n) mod 11907]) + 2^14 >> 15 )
@@ -18,12 +18,17 @@
 //              the rows overlap - row n+1 starts 64 bytes after row n - so the capture is addressed as a [rows][64 B]
 //              matrix and K chunk c of row n is matrix row n + c: eight TMA boxes per tile, no im2col pass)
 //   B[r][.]  = per channel four rows: {real, imaginary} x {high, low byte} of the 16-bit taps (signed 8-bit; the
-//              real row holds Wr, -Wi alternating, the imaginary row Wi, Wr)
-//   D        = int32 in TMEM; acc = 256 * D_high + D_low - 127 * (sum of the row), the last term a per-channel constant
-// tcgen05.mma.kind::i8, M = 128 output samples x N = 128 rows (32 channels) x K = 512 per tile; one persistent CTA per
-// (channel group, tile slot): warp 0 = TMA producer, warp 1 = MMA issuer, warps 2..5 = epilogue (TMEM -> registers ->
-// rounding, rotation, saturation -> coalesced cs16 stores).  The 32 channels' taps (64 KB) stay in shared memory for the
-// CTA's lifetime; capture tiles are double-buffered (2 x 64 KB), accumulators double-buffered in TMEM (2 x 128 columns).
+//              real row holds Wr, -Wi alternating, the imaginary row Wi, Wr).  Channel cl = 4 p + q of the group owns
+//              rows 16 p + 2 q + {0: real, 1: imaginary} (high bytes) and the same + 8 (low bytes): in the wgmma
+//              accumulator layout, where lane q = lane % 4 holds columns 8 j + 2 q, +1 of every 8-column block j,
+//              one thread then holds all four sums of its channels and the epilogue needs no shuffles.
+//   D        = int32 in registers; acc = 256 * D_high + D_low - 127 * (sum of the row), the last term a per-channel constant
+// Hopper wgmma (u8 x s8 -> s32), M = 64 output samples x N = 128 rows (32 channels) x K = 512 per tile, both operands
+// K-major in shared memory with the 64-byte swizzle.  One persistent CTA per (channel group, tile slot), three
+// warpgroups: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that take the CTA's tiles in
+// turn, each issuing its tile's 16 wgmmas and then running the epilogue from its own registers (rounding, rotation,
+// saturation -> cs16 stores) while the other consumer's wgmmas run.  The 32 channels' taps (64 KB) stay in shared
+// memory for the CTA's lifetime; capture tiles go through a ring of four 32 KB stages.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -40,17 +45,19 @@ namespace nbch {
 
 constexpr int DECIM = 32, TAPS = 256, KBYTES = 2 * TAPS;          // 512 bytes of K per output row
 constexpr int CHUNK = 64, NCHUNK = KBYTES / CHUNK;               // K chunks of 64 bytes (one capture-matrix row each)
-constexpr int TILE_M = 128;                                       // output samples per tile
+constexpr int TILE_M = 64;                                        // output samples per tile (one warpgroup's wgmma M)
 constexpr int GROUP = 32, TILE_N = 4 * GROUP;                    // channels per CTA, rows of B
 constexpr int PERIOD = 11907;                                     // phasor table length (100 kHz / 23.814 MHz = 50 / 11907)
 constexpr int SHIFT1 = 13, TAP_SCALE_LOG2 = 19;                   // unit DC gain -> 64 LSB per input LSB (the cu8 -> Q15 convention);
                                                                   // taps stay below 127 * 256 + 127: both bytes of the split are int8
-constexpr int THREADS = 192;
-constexpr uint32_t A_STAGE_BYTES = NCHUNK * TILE_M * CHUNK;      // 65536
+constexpr int THREADS = 384;                                      // producer warpgroup + two consumer warpgroups
+constexpr int STAGES = 4;
+constexpr uint32_t A_STAGE_BYTES = NCHUNK * TILE_M * CHUNK;      // 32768
 constexpr uint32_t W_BYTES = NCHUNK * TILE_N * CHUNK;            // 65536
 constexpr int HALF = PERIOD / 2 + 1;                              // phasor table entries 0 .. 5953; the rest are their conjugates
 constexpr uint32_t EPI_BYTES = ((HALF * 4 + 15) & ~15) + GROUP * 4 + 2 * GROUP * 4;   // half table, rotation steps, offset corrections
-constexpr uint32_t SMEM_BYTES = W_BYTES + 2 * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
+constexpr uint32_t SMEM_BYTES = W_BYTES + STAGES * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
+static_assert(SMEM_BYTES <= 227 * 1024, "more shared memory than an H100 block may have");
 
 struct Params {
     int nch;                   // channels
@@ -99,36 +106,40 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
                  : "memory");
 }
 // K-major operand tile in shared memory, 64-byte rows, SWIZZLE_64B: 8-row groups 512 bytes apart
-__device__ __forceinline__ uint64_t umma_desc_sw64(const void *tile, uint32_t byte_offset)
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(const void *tile, uint32_t byte_offset)
 {
     const uint32_t addr = smem_u32(tile) + byte_offset;
     uint64_t d = 0;
     d |= (uint64_t)((addr & 0x3FFFFu) >> 4);                 // start address
     d |= (uint64_t)1 << 16;                                    // leading byte offset (unused for swizzled K-major): 1
     d |= (uint64_t)(512u >> 4) << 32;                          // stride byte offset: 8 rows x 64 B
-    d |= (uint64_t)1 << 46;                                    // descriptor version (Blackwell)
-    d |= (uint64_t)4 << 61;                                    // layout type SWIZZLE_64B
+    d |= (uint64_t)2 << 62;                                    // layout type SWIZZLE_64B
     return d;
 }
-// instruction descriptor, kind::i8: D = S32, A = unsigned 8-bit (capture bytes), B = signed 8-bit (taps), both K-major
-constexpr uint32_t IDESC = (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(TILE_N >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24);
-
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate)
+// D (64 x 128 int32, this thread's 64 of them) += A (64 x 32 capture bytes, unsigned) * B (128 x 32 tap bytes, signed)^T;
+// accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_u8s8(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate)
 {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(IDESC), "r"(accumulate), "r"(0u)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate)
         : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 struct Barriers {
-    uint64_t w_full, a_full[2], a_empty[2], d_full[2], d_empty[2];
-    uint32_t tmem_base;
+    uint64_t w_full, a_full[STAGES], a_empty[STAGES];
 };
 
 __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
@@ -137,11 +148,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t *smem_w = smem;                                        // [8 chunks][128 rows][64 B]
-    uint8_t *smem_a = smem + W_BYTES;                              // [2 stages][8 chunks][128 rows][64 B]
-    Barriers &bar = *reinterpret_cast<Barriers *>(smem + W_BYTES + 2 * A_STAGE_BYTES);
+    uint8_t *smem_a = smem + W_BYTES;                              // [STAGES][8 chunks][64 rows][64 B]
+    Barriers &bar = *reinterpret_cast<Barriers *>(smem + W_BYTES + STAGES * A_STAGE_BYTES);
     // the epilogue's tables in shared memory: the first half of the phasor table (P[11907 - i] = conj(P[i]), made so on
     // the host), and this group's rotation steps and offset corrections
-    short2 *ph_half = reinterpret_cast<short2 *>(smem + W_BYTES + 2 * A_STAGE_BYTES + 256);
+    short2 *ph_half = reinterpret_cast<short2 *>(smem + W_BYTES + STAGES * A_STAGE_BYTES + 256);
     int *s_rot = reinterpret_cast<int *>(reinterpret_cast<uint8_t *>(ph_half) + ((HALF * 4 + 15) & ~15));
     uint32_t *s_corr = reinterpret_cast<uint32_t *>(s_rot + GROUP);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -149,127 +160,91 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
 
     for (int i = threadIdx.x; i < HALF; i += THREADS) ph_half[i] = p.phasor[i];
     for (int i = threadIdx.x; i < GROUP; i += THREADS) {
-        const int ch = min(((int)blockIdx.x % p.ngroups) * GROUP + i, p.nch - 1);
+        const int ch = min(group * GROUP + i, p.nch - 1);
         s_rot[i] = p.rot_step[ch];
         s_corr[2 * i] = (uint32_t)p.corr[2 * ch];
         s_corr[2 * i + 1] = (uint32_t)p.corr[2 * ch + 1];
     }
     if (threadIdx.x == 0) {
         mbar_init(&bar.w_full, 1);
-        for (int i = 0; i < 2; i++) {
+        for (int i = 0; i < STAGES; i++) {
             mbar_init(&bar.a_full[i], 1);
-            mbar_init(&bar.a_empty[i], 1);
-            mbar_init(&bar.d_full[i], 1);
-            mbar_init(&bar.d_empty[i], 4);                         // one arrival per epilogue warp
+            mbar_init(&bar.a_empty[i], 4);                         // one arrival per warp of the consuming warpgroup
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {                                               // TMEM: 2 x 128 columns of int32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bar.tmem_base)), "n"(256));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    const uint32_t tmem_base = bar.tmem_base;
 
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
+    const int wgi = __shfl_sync(0xffffffffu, threadIdx.x / 128, 0);   // warpgroup index, known to be warp-uniform
+    if (wgi == 0) {
+        // ===== TMA producer (one thread) =====
+        if (threadIdx.x == 0) {
             mbar_expect_tx(&bar.w_full, W_BYTES);
             for (int c = 0; c < NCHUNK; c++)
                 tma_load_2d(smem_w + (size_t)c * TILE_N * CHUNK, &map_w, &bar.w_full, 0, (group * NCHUNK + c) * TILE_N);
             unsigned it = 0;
             for (long long tile = slot; tile < p.tiles; tile += nslots, it++) {
-                const int s = it & 1;
-                if (it >= 2) mbar_wait(&bar.a_empty[s], ((it >> 1) - 1) & 1);
+                const int s = it % STAGES;
+                if (it >= STAGES) mbar_wait(&bar.a_empty[s], (it / STAGES - 1) & 1);
                 mbar_expect_tx(&bar.a_full[s], A_STAGE_BYTES);
                 for (int c = 0; c < NCHUNK; c++)                 // K chunk c of output row n = capture-matrix row n + c
                     tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, &map_x, &bar.a_full[s], 0,
                                 (int)(tile * TILE_M) + c);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            mbar_wait(&bar.w_full, 0);
-            unsigned it = 0;
-            for (long long tile = slot; tile < p.tiles; tile += nslots, it++) {
-                const int s = it & 1;
-                if (it >= 2) mbar_wait(&bar.d_empty[s], ((it >> 1) - 1) & 1);       // the epilogue has drained this accumulator
-                mbar_wait(&bar.a_full[s], (it >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;");
-                const uint32_t tmem_d = tmem_base + (uint32_t)s * TILE_N;
-                for (int c = 0; c < NCHUNK; c++)
-                    for (int k = 0; k < CHUNK / 32; k++) {       // UMMA K = 32 bytes
-                        const uint64_t da = umma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
-                        const uint64_t db = umma_desc_sw64(smem_w + (size_t)c * TILE_N * CHUNK, 32u * k);
-                        umma_i8(tmem_d, da, db, (c | k) ? 1u : 0u);
-                    }
-                umma_commit(&bar.a_empty[s]);                     // shared-memory stage free once these MMAs have read it
-                umma_commit(&bar.d_full[s]);                      // accumulator complete
+        return;
+    }
+    // ===== consumers: warpgroup 1 takes the CTA's even tiles, warpgroup 2 the odd ones =====
+    const int wg = wgi - 1, wwarp = warp & 3;
+    const int q = lane & 3;                                        // this thread's channels: cl = 4 i + q, i = 0 .. 7
+    mbar_wait(&bar.w_full, 0);
+    unsigned it = (unsigned)wg;
+    for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2) {
+        const int s = it % STAGES;
+        mbar_wait(&bar.a_full[s], (it / STAGES) & 1);
+        uint32_t d[64];                                            // (the first wgmma overwrites it: accumulate = 0)
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+        for (int c = 0; c < NCHUNK; c++)
+#pragma unroll
+            for (int k = 0; k < CHUNK / 32; k++) {                 // wgmma K = 32 bytes
+                const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
+                const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)c * TILE_N * CHUNK, 32u * k);
+                wgmma_u8s8(d, da, db, (c | k) ? 1u : 0u);
             }
-        }
-    } else {
-        // ===== epilogue: warp w reads TMEM lanes 32 (w % 4) .. +31 = tile rows =====
-        const int quarter = warp & 3;
-        const int row = 32 * quarter + lane;
-        unsigned it = 0;
-        for (long long tile = slot; tile < p.tiles; tile += nslots, it++) {
-            const int s = it & 1;
-            mbar_wait(&bar.d_full[s], (it >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;");
-            const long long n = tile * TILE_M + row;
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bar.a_empty[s]);               // the stage's bytes are no longer needed
+
+        // ===== epilogue: rows 16 wwarp + lane / 4 (h = 0) and + 8 (h = 1) of the tile =====
+        // 32-bit arithmetic throughout: 256 * hi + lo wraps, the filter output itself is bounded by
+        // 128 * sum(|Wr| + |Wi|) < 2^28 (checked when the tables are made), so the wrapped sum is the value; after
+        // the shift a component is below 2^15 and the rotation's two products stay below 2^31.
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const long long n = tile * TILE_M + 16 * wwarp + (lane >> 2) + 8 * h;
             const int nmod = (int)(n % PERIOD);
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * quarter) << 16) + (uint32_t)s * TILE_N;
-#pragma unroll 1
-            for (int c0 = 0; c0 < GROUP; c0 += 8) {              // 8 channels = 32 columns per load
-                uint32_t v[32];
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                      "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                      "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr + 4u * c0));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                // 32-bit arithmetic throughout: 256 * hi + lo wraps, the filter output itself is bounded by
-                // 128 * sum(|Wr| + |Wi|) < 2^28 (checked when the tables are made), so the wrapped sum is the value; after
-                // the shift a component is below 2^15 and the rotation's two products stay below 2^31.  No branches: the
-                // eight table reads of a load are independent and go out together.
-                short2 ph[8];
 #pragma unroll
-                for (int q = 0; q < 8; q++) {
-                    const unsigned qi = ((unsigned)s_rot[c0 + q] * (unsigned)nmod) % (unsigned)PERIOD;   // < 11907^2 < 2^32
-                    const bool up = qi >= (unsigned)HALF;
-                    const short2 v2 = ph_half[up ? (unsigned)PERIOD - qi : qi];
-                    ph[q] = make_short2(v2.x, up ? (short)-v2.y : v2.y);
-                }
-#pragma unroll
-                for (int q = 0; q < 8; q++) {
-                    const int ch = group * GROUP + c0 + q;
-                    const int ar = (int)(256u * v[4 * q + 0] + v[4 * q + 2] - s_corr[2 * (c0 + q)]);
-                    const int ai = (int)(256u * v[4 * q + 1] + v[4 * q + 3] - s_corr[2 * (c0 + q) + 1]);
-                    const int vr = (ar + (1 << (SHIFT1 - 1))) >> SHIFT1, vi = (ai + (1 << (SHIFT1 - 1))) >> SHIFT1;
-                    int zr = vr * ph[q].x + vi * ph[q].y, zi = vi * ph[q].x - vr * ph[q].y;    // v * conj(P)
-                    zr = (zr + (1 << 14)) >> 15;
-                    zi = (zi + (1 << 14)) >> 15;
-                    zr = zr > 32767 ? 32767 : (zr < -32768 ? -32768 : zr);
-                    zi = zi > 32767 ? 32767 : (zi < -32768 ? -32768 : zi);
-                    const uint32_t packed = (uint32_t)(uint16_t)(int16_t)zr | ((uint32_t)(uint16_t)(int16_t)zi << 16);
-                    if (ch < p.nch && n < p.nout) *reinterpret_cast<uint32_t *>(p.out + (size_t)ch * p.out_stride + 2 * n) = packed;
-                }
+            for (int i = 0; i < 8; i++) {
+                const int cl = 4 * i + q, ch = group * GROUP + cl;
+                const unsigned qi = ((unsigned)s_rot[cl] * (unsigned)nmod) % (unsigned)PERIOD;   // < 11907^2 < 2^32
+                const bool up = qi >= (unsigned)HALF;
+                const short2 v2 = ph_half[up ? (unsigned)PERIOD - qi : qi];
+                const int phx = v2.x, phy = up ? -v2.y : v2.y;
+                const int ar = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h] - s_corr[2 * cl]);
+                const int ai = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h] - s_corr[2 * cl + 1]);
+                const int vr = (ar + (1 << (SHIFT1 - 1))) >> SHIFT1, vi = (ai + (1 << (SHIFT1 - 1))) >> SHIFT1;
+                int zr = vr * phx + vi * phy, zi = vi * phx - vr * phy;        // v * conj(P)
+                zr = (zr + (1 << 14)) >> 15;
+                zi = (zi + (1 << 14)) >> 15;
+                zr = zr > 32767 ? 32767 : (zr < -32768 ? -32768 : zr);
+                zi = zi > 32767 ? 32767 : (zi < -32768 ? -32768 : zi);
+                const uint32_t packed = (uint32_t)(uint16_t)(int16_t)zr | ((uint32_t)(uint16_t)(int16_t)zi << 16);
+                if (ch < p.nch && n < p.nout) *reinterpret_cast<uint32_t *>(p.out + (size_t)ch * p.out_stride + 2 * n) = packed;
             }
-            asm volatile("tcgen05.fence::before_thread_sync;");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar.d_empty[s]);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(256));
 }
 
 }  // namespace nbch
@@ -339,6 +314,7 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
         if (rot) (*rot)[k] = (int)((((long long)1600 * m) % PERIOD + PERIOD) % PERIOD);
         long long swr = 0, swi = 0, sabs = 0;
         const int g = k / GROUP, cl = k % GROUP;
+        const int brow = 16 * (cl / 4) + 2 * (cl % 4);                   // B rows of the channel: brow + part (+ 8: low bytes)
         for (int u = 0; u < TAPS; u++) {
             // W_k[u] = 2^19 h[255-u] e^{-j 2 pi 50 m u / 11907}, from the integer phasor table
             const short2 ph = phasor[(size_t)((step * u) % PERIOD)];
@@ -359,8 +335,8 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
                     if (hi < -128 || hi > 127) { fprintf(stderr, "nrsc5_b200: channeliser tap out of range\n"); abort(); }
                     const int kappa = 2 * u + comp, ck = kappa / CHUNK, b = kappa % CHUNK;
                     const size_t base = ((size_t)(g * NCHUNK + ck) * TILE_N) * CHUNK;
-                    (*w)[base + (size_t)(4 * cl + part) * CHUNK + b] = (int8_t)hi;
-                    (*w)[base + (size_t)(4 * cl + 2 + part) * CHUNK + b] = (int8_t)lo;
+                    (*w)[base + (size_t)(brow + part) * CHUNK + b] = (int8_t)hi;
+                    (*w)[base + (size_t)(brow + 8 + part) * CHUNK + b] = (int8_t)lo;
                 }
         }
         // the kernel's epilogue computes in 32 bits (k_channelize): the filter output must stay below 2^28
@@ -489,7 +465,7 @@ extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8
     p.rot_step = c->d_rot;
     p.corr = c->d_corr;
     p.phasor = c->d_phasor;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
     long long slots = sms / c->ngroups;
     if (slots < 1) slots = 1;

@@ -1,4 +1,4 @@
-// Shared definitions for the nrsc5_b200 CUDA engine (sm_100a).
+// Shared definitions for the nrsc5_b200 CUDA engine (sm_90a).
 //
 // Vocabulary follows the reference domain: a *stream* is one independent
 // radio channel (one nrsc5_t in the reference); a *block* is 32 OFDM symbols

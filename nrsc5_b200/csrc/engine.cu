@@ -893,7 +893,7 @@ static void launch_k_stream(nrsc5b_engine *e, int last_pass);
 
 extern "C" int nrsc5b_debug_set(int flags);
 
-extern "C" const char *nrsc5b_version(void) { return "nrsc5_b200 0.1 (sm_100a)"; }
+extern "C" const char *nrsc5b_version(void) { return "nrsc5_b200 0.1 (sm_90a)"; }
 
 extern "C" int nrsc5b_create(nrsc5b_engine_t **out, const nrsc5b_config_t *cfg)
 {
@@ -987,7 +987,7 @@ extern "C" int nrsc5b_create(nrsc5b_engine_t **out, const nrsc5b_config_t *cfg)
     {
         // fast Viterbi: one thread per chunk; pick the chunk length so that the warps of all streams' frames
         // make one wave over the GPU's warp schedulers (4 per SM)
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
         int wpf = (4 * sms) / S;
         if (wpf < 1) wpf = 1;
@@ -1164,7 +1164,7 @@ extern "C" int nrsc5b_create(nrsc5b_engine_t **out, const nrsc5b_config_t *cfg)
 #if !defined(NB_EMU)
     if (cfg->mode == NRSC5B_MODE_FM) {
         // fewer streams than SMs: a cluster of 4 or 2 CTAs per stream shares the demodulation of every block
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
         const char *force = getenv("NRSC5_B200_CLUSTER");
         for (int c = 4; c >= 2; c >>= 1) {

@@ -1,7 +1,7 @@
 /* bench_pipe: one capture through the PUBLIC libnrsc5 API exactly as the reference's CLI feeds a file
  * (reference src/main.c:1097-1119: fread 32 768 bytes -> nrsc5_pipe_samples_cu8, then nrsc5_stop / nrsc5_close),
  * with the library given on the command line and loaded with dlopen - so the very same binary times the drop-in
- * (nrsc5_b200/dropin/_build/libnrsc5.so, B200 engine underneath) and the unmodified reference
+ * (nrsc5_b200/dropin/_build/libnrsc5.so, CUDA engine underneath) and the unmodified reference
  * (oracle/_ref/libnrsc5_ref.so, CPU) on the same bytes.  Prints one JSON object: wall seconds of the push loop
  * (input already in memory; open and close outside / inside as stated), event counts and an FNV-1a digest of all
  * HDC packets so that the two runs can be compared.

@@ -1,5 +1,5 @@
 /* input.h of the drop-in libnrsc5.so: the seam between the reference's unmodified host side (nrsc5.c,
- * frame.c, pids.c, output.c, ... compiled from the reference tree as they are) and the B200 engine.
+ * frame.c, pids.c, output.c, ... compiled from the reference tree as they are) and the CUDA engine.
  *
  * It replaces reference src/input.h:1-43.  The host side only ever touches four members of input_t -
  * `radio`, `output`, `frame` (frame.c:746, decode.c:460) and, through pids_init(), `pids` - and calls the

@@ -1,5 +1,5 @@
 /* The seven input_* functions of the reference (src/input.c:96-188, declared src/input.h:37-43) on top of
- * the B200 engine's C ABI (include/nrsc5_b200.h).  Linked with the reference's unmodified host-side
+ * the CUDA engine's C ABI (include/nrsc5_b200.h).  Linked with the reference's unmodified host-side
  * sources this gives a libnrsc5.so whose public API and event order are the reference's.
  *
  * input_push_cu8() never waits for the GPU: it copies the samples into the engine's page-locked staging area
@@ -42,7 +42,7 @@
 
 static void fail(const char *what, int rc)
 {
-    fprintf(stderr, "libnrsc5 (B200): %s failed (%d); there is no CPU path\n", what, rc);
+    fprintf(stderr, "libnrsc5 (GPU): %s failed (%d); there is no CPU path\n", what, rc);
     abort();
 }
 
@@ -434,12 +434,12 @@ void input_free(input_t *st)
         pump_all(st);
     const double t1 = st->trace ? seam_now() : 0;
     if (st->trace)
-        fprintf(stderr, "libnrsc5 (B200) trace: %lu batches delivered, %lu record bytes, %.6f s in the replay (callbacks included), "
+        fprintf(stderr, "libnrsc5 (GPU) trace: %lu batches delivered, %lu record bytes, %.6f s in the replay (callbacks included), "
                         "%.6f s in the final flush\n", st->trace_batches, st->trace_bytes, st->trace_replay_s, t1 - t0);
     frame_free(&st->frame);
     nrsc5b_destroy(st->engine);
     if (st->trace)
-        fprintf(stderr, "libnrsc5 (B200) trace: %.6f s in nrsc5b_destroy\n", seam_now() - t1);
+        fprintf(stderr, "libnrsc5 (GPU) trace: %.6f s in nrsc5b_destroy\n", seam_now() - t1);
     free(st->records);
     free(st->bits);
 }

@@ -9,9 +9,22 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 SAMPLE_CANDIDATES = [
-    os.path.join(ROOT, "oracle", "_ref", "sample.xz"),   # copied there by build(); travels to the GPU box
-    "/root/reference/support/sample.xz",
+    os.path.join(ROOT, "oracle", "_ref", "sample.xz"),   # copied there by build() from the reference tree
 ]
+
+
+def dropin_objects():
+    """The drop-in libnrsc5.so's objects without the engine: the reference's host-side units (oracle/_ref/dropin/obj)
+    and our seam and rtl-sdr stub, compiled - and checked to agree on input.h - by nrsc5_b200/dropin/Makefile.  None when
+    oracle/_ref/dropin has not been built."""
+    import glob
+    import subprocess
+    ref = os.path.join(ROOT, "oracle", "_ref", "dropin", "obj")
+    if not os.path.exists(os.path.join(ref, "input_h.sha256")):
+        return None
+    own = ["_build/obj/ref_objs_match", "_build/obj/seam_input_seam.o", "_build/obj/shim_rtlstub.o"]
+    subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "nrsc5_b200", "dropin"), *own], check=True)
+    return sorted(glob.glob(os.path.join(ref, "*.o"))) + [os.path.join(ROOT, "nrsc5_b200", "dropin", p) for p in own[1:]]
 
 
 def fnv1a32(b: bytes) -> int:

@@ -10,9 +10,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "gpu_new: needs a CUDA device; verified on the CPU emulation of the kernels "
-                                       "(tests/test_emu_engine.py) but not yet run on a B200 - select with -m 'gpu or gpu_new'")
+                                       "(tests/test_emu_engine.py) but not yet run on a GPU - select with -m 'gpu or gpu_new'")
 
 
 def _have_gpu():

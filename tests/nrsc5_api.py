@@ -1,6 +1,6 @@
 """Minimal ctypes driver of the reference's PUBLIC API (reference include/nrsc5.h: nrsc5_open_pipe,
 nrsc5_set_callback, nrsc5_pipe_samples_cu8, nrsc5_close) - test infrastructure.  It is pointed either at
-the unmodified reference (oracle/_ref/libnrsc5_ref.so) or at the drop-in built on the B200 engine
+the unmodified reference (oracle/_ref/libnrsc5_ref.so) or at the drop-in built on the CUDA engine
 (nrsc5_b200/dropin/_build/libnrsc5.so) and digests the events both deliver through the same callback.
 
 Event layout (nrsc5.h:369-613): `unsigned int event` followed by a union aligned to 8 bytes.

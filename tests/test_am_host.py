@@ -24,7 +24,7 @@ def _lib():
            os.path.join(common.ROOT, "nrsc5_b200", "csrc", "am_tables.h")]
     if not os.path.exists(SO) or any(os.path.getmtime(p) > os.path.getmtime(SO) for p in src):
         os.makedirs(os.path.dirname(SO), exist_ok=True)
-        subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "--expt-extended-lambda", "--expt-relaxed-constexpr", "-O2", "-shared", "-Xcompiler", "-fPIC", "-o", SO,
+        subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "--expt-extended-lambda", "--expt-relaxed-constexpr", "-O2", "-shared", "-Xcompiler", "-fPIC", "-o", SO,
                         src[0], "-L" + os.path.join(common.ROOT, "oracle", "_ref"), "-loracle",
                         "-Xlinker", "-rpath", "-Xlinker", os.path.join(common.ROOT, "oracle", "_ref")], check=True)
     L = ctypes.CDLL(SO)

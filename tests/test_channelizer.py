@@ -1,5 +1,5 @@
 """Wideband channeliser (SURVEY 8 f3; csrc/channelizer.cu).  CPU tier: the definition's tables (filter quality) and its
-numpy restatement on signals with known answers.  GPU tier: the tcgen05 kernel against the restatement, bit for bit,
+numpy restatement on signals with known answers.  GPU tier: the wgmma kernel against the restatement, bit for bit,
 and end to end - stations mixed into a 23.814 MS/s capture come out of channeliser + engine with their PDUs intact."""
 import numpy as np
 import pytest

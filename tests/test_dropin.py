@@ -1,4 +1,4 @@
-"""The drop-in libnrsc5.so (reference host side + our input seam + the B200 engine) driven through the
+"""The drop-in libnrsc5.so (reference host side + our input seam + the CUDA engine) driven through the
 reference's PUBLIC API must deliver the events the unmodified reference delivers - same kinds, same order,
 identical HDC audio packets - on support/sample.xz (golden: tests/golden/api_sample_xz.json, made by
 tests/golden/make_golden_api.py with the unmodified reference)."""
@@ -20,7 +20,7 @@ PUBLIC_API = ["nrsc5_get_version", "nrsc5_service_data_type_name", "nrsc5_progra
 
 def test_dropin_exports_the_public_api():
     if not os.path.exists(DROPIN):
-        pytest.skip("drop-in not built (needs the reference tree at build time)")
+        pytest.skip("drop-in not built (its reference-side objects in oracle/_ref/ are missing)")
     out = subprocess.run(["nm", "-D", "--defined-only", DROPIN], capture_output=True, text=True).stdout
     names = {ln.split()[-1] for ln in out.splitlines() if ln.strip()}
     for n in PUBLIC_API:

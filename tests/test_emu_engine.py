@@ -7,7 +7,7 @@ What this proves and what it does not: the kernels' logic - indexing, work split
 divergent barrier deadlocks the emulator, which reports it instead of hanging a device), the host side of the C
 ABI - is exercised bit for bit against the oracle on the CPU tier.  It says nothing about speed, and floating
 point can differ from the GPU's in the last place (glibc's sincosf/atan2f, exact instead of approximate division),
-so the `-m gpu` run of the same tests on a B200 remains the parity gate.  The emulator is test infrastructure: the
+so the `-m gpu` run of the same tests on an H100 remains the parity gate.  The emulator is test infrastructure: the
 product library (nrsc5_b200/build.py, nvcc) has no CPU path.
 """
 import os
@@ -56,7 +56,7 @@ test_viterbi_k9_equals_the_reference_decoder = _stages.test_viterbi_k9_equals_th
 
 
 def test_rs_beyond_the_correction_radius_equals_reference():
-    nfail, ncorr = _stages.rs_beyond_radius(6000)         # (120 000 words on the B200)
+    nfail, ncorr = _stages.rs_beyond_radius(6000)         # (120 000 words on the GPU)
     assert nfail > 5000
 
 
@@ -115,10 +115,9 @@ def test_reverse_thread_order_gives_the_same_results():
 def emulated_dropin(emulated_engine):
     import build_emu
     import test_dropin
-    objdir = os.path.join(common.ROOT, "nrsc5_b200", "dropin", "_build", "obj")
-    if not os.path.isdir(objdir):
-        pytest.skip("drop-in objects not built (needs the reference tree at build time)")
-    objs = sorted(os.path.join(objdir, f) for f in os.listdir(objdir) if f.endswith(".o"))
+    objs = common.dropin_objects()
+    if objs is None:
+        pytest.skip("drop-in objects not built (oracle/_ref/ is built where the reference tree is)")
     so = os.path.join(HERE, "_build", "libnrsc5_emu.so")
     emu = build_emu.build()
     subprocess.run(["gcc", "-shared", "-o", so, *objs, emu, "-Wl,-rpath," + os.path.dirname(emu), "-lm", "-lpthread"], check=True)
@@ -128,7 +127,7 @@ def emulated_dropin(emulated_engine):
     test_dropin.DROPIN = saved
 
 
-@pytest.mark.parametrize("device_l2", [1])       # 0 (the reference's frame.c on the host) is the path the B200 run covers
+@pytest.mark.parametrize("device_l2", [1])       # 0 (the reference's frame.c on the host) is the path the GPU run covers
 def test_dropin_events_match_reference_on_sample_xz(emulated_dropin, device_l2):
     import test_dropin
     test_dropin.test_dropin_events_match_reference_on_sample_xz(device_l2)

@@ -1,7 +1,7 @@
 """GPU parity of the AM (hybrid MA1, all-digital MA3) path through the C ABI: cs16 in, P1 / P3 / PIDS PDUs and events out, against
 the oracle (oracle/nrsc5_oracle_am.c, itself pinned to the unmodified reference) and the golden vectors.
 
-First B200 run: round 1, all green (they ran as `gpu_new` until then; their CPU twins on the emulated kernels
+First GPU run: round 1, all green (they ran as `gpu_new` until then; their CPU twins on the emulated kernels
 are in tests/test_emu_engine.py)."""
 import numpy as np
 import pytest

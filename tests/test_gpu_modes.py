@@ -1,7 +1,7 @@
 """GPU parity of the FM service modes beyond MP1 / MP3 through the C ABI: MP2, MP5, MP6, MP11 against the oracle and
 the golden vectors of the unmodified reference (tests/golden/synth_fm_modes.json).
 
-First B200 run: round 1, all green (they ran as `gpu_new` until then; their CPU twins on the emulated kernels
+First GPU run: round 1, all green (they ran as `gpu_new` until then; their CPU twins on the emulated kernels
 are in tests/test_emu_engine.py)."""
 import numpy as np
 import pytest

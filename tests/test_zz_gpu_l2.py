@@ -4,7 +4,7 @@ golden call streams made from the reference (tests/golden/l2.json).  Through the
 alone, all six frame lengths) and nrsc5b_enable_l2 (the whole chain, REC_L2 after every frame's pass).
 
 They went green on the CPU emulation of the kernels first (tests/test_emu_engine.py runs these very functions) and
-then on the B200 (profiles/r1_l2_gpu_tests.txt)."""
+then on the GPU."""
 import os
 
 import pytest

@@ -4,16 +4,17 @@
     cat sample | nrsc5 -r - -o sample.wav 0       ; same grep
     support/cli.py -r sample -o sample.wav 0      ; same grep
 
-with `nrsc5` = the reference's UNMODIFIED command-line program (src/main.c + src/log.c, compiled where they lie by
-tests/cli/build_cli.py, libao replaced by a byte-counting stand-in) linked against the drop-in libnrsc5.so, and
+with `nrsc5` = the reference's UNMODIFIED command-line program (src/main.c + src/log.c, compiled into
+oracle/_ref/cli/ and linked by tests/cli/build_cli.py, libao replaced by a byte-counting stand-in) linked against the drop-in libnrsc5.so, and
 `support/cli.py` = the reference's unmodified Python CLI loading the drop-in through its own ctypes binding
 (support/nrsc5.py:676-690).  This is the claim of BASELINE.json's north_star - "the CLI and Python bindings drop in
 unchanged" - tested the way the reference tests itself.  Beyond the grep, every information line the CLI prints
 (station, audio services, titles, artists, ...) must equal, in order, what the same program prints when linked
-against the unmodified reference library.
+against the unmodified reference library (stored in tests/golden/cli_sample_xz.json).
 
 CPU tier: the drop-in on the CPU emulation of the kernels (tests/emu), first 20 MB of the capture.
-GPU tier: the real drop-in, whole capture; the binaries are built by __graft_entry__.build() and travel to the box.
+GPU tier: the real drop-in, whole capture; the binaries are built by __graft_entry__.build() (the reference-side
+objects in oracle/_ref/).
 """
 import os
 import re
@@ -31,7 +32,8 @@ import build_cli  # noqa: E402
 
 BUILD = os.path.join(HERE, "_build")
 GREP = "You're Listening to Q"
-REF_SUPPORT = "/root/reference/support"
+PREFIX_BYTES = 20_000_000
+REF_SUPPORT = os.path.join(common.ROOT, "oracle", "_ref", "support")   # the reference's Python CLI, copied by build()
 
 
 def info_lines(log: str):
@@ -53,7 +55,7 @@ def sample_files(tmp_path_factory):
     d = tmp_path_factory.mktemp("cli")
     full, part = d / "sample", d / "sample20"
     full.write_bytes(raw.tobytes())
-    part.write_bytes(raw.tobytes()[:20_000_000])
+    part.write_bytes(raw.tobytes()[:PREFIX_BYTES])
     return str(full), str(part), str(d)
 
 
@@ -68,26 +70,25 @@ def run_cli(binary, sample, workdir, stdin=False):
     return r.stderr
 
 
-def control_binary():
-    import reftap
-    p = os.path.join(BUILD, "nrsc5_ref")
-    if build_cli.available() and reftap.available():
-        return build_cli.build(reftap.REF_SO, "ref")
-    return p if os.path.exists(p) else None
+def control(key):
+    """What the same program prints when linked against the unmodified reference library (tests/golden/cli_sample_xz.json,
+    made by tests/golden/make_golden_cli.py)."""
+    g = common.golden("cli_sample_xz.json")
+    assert common.fnv1a32(common.load_sample()[:1 << 20].tobytes()) == g["input_fnv"]
+    return g[key]
 
 
 @pytest.fixture(scope="module")
 def emulated_cli():
     """libnrsc5.so = the drop-in's objects on the emulated engine, and the reference CLI linked against it."""
     import build_emu
-    objdir = os.path.join(common.ROOT, "nrsc5_b200", "dropin", "_build", "obj")
-    if not build_cli.available() or not os.path.isdir(objdir):
-        pytest.skip("needs the reference tree (the CLI and the drop-in's host objects are compiled from it)")
+    objs = common.dropin_objects()
+    if not build_cli.available() or objs is None:
+        pytest.skip("needs oracle/_ref/ built where the reference tree is (the CLI and the drop-in's host objects)")
     emu = build_emu.build()
     libdir = os.path.join(BUILD, "emu_lib")
     os.makedirs(libdir, exist_ok=True)
     so = os.path.join(libdir, "libnrsc5.so")
-    objs = sorted(os.path.join(objdir, f) for f in os.listdir(objdir) if f.endswith(".o"))
     subprocess.run(["gcc", "-shared", "-o", so, *objs, emu, "-Wl,-rpath," + os.path.dirname(emu), "-lm", "-lpthread"], check=True)
     return build_cli.build(so, "emu"), libdir
 
@@ -97,9 +98,7 @@ def test_reference_cli_on_the_emulated_dropin(emulated_cli, sample_files):
     _, part, work = sample_files
     log = run_cli(binary, part, work)
     assert GREP in log                                              # ci.yml:35
-    ctl = control_binary()
-    assert ctl is not None
-    assert info_lines(log) == info_lines(run_cli(ctl, part, work)) and len(info_lines(log)) >= 8
+    assert info_lines(log) == control("prefix_20mb") and len(info_lines(log)) >= 8
 
 
 def test_reference_python_cli_on_the_emulated_dropin(emulated_cli, sample_files):
@@ -107,7 +106,7 @@ def test_reference_python_cli_on_the_emulated_dropin(emulated_cli, sample_files)
     _, libdir = emulated_cli
     _, part, work = sample_files
     if not os.path.exists(os.path.join(REF_SUPPORT, "cli.py")):
-        pytest.skip("reference tree not present")
+        pytest.skip("the reference's support/cli.py is not in oracle/_ref/")
     env = dict(os.environ, PYTHONPATH=os.path.join(HERE, "cli", "stubs") + os.pathsep + REF_SUPPORT,
                LD_LIBRARY_PATH=libdir + os.pathsep + os.environ.get("LD_LIBRARY_PATH", ""))
     with open(part, "rb") as f:
@@ -125,11 +124,9 @@ def test_reference_cli_on_the_dropin(sample_files, stdin):
     if build_cli.available():
         binary = build_cli.build(os.path.join(common.ROOT, "nrsc5_b200", "dropin", "_build", "libnrsc5.so"), "dropin")
     if not os.path.exists(binary):
-        pytest.skip("reference CLI not built (needs the reference tree at build time)")
+        pytest.skip("reference CLI not built (oracle/_ref/ is built where the reference tree is)")
     full, _, work = sample_files
     log = run_cli(binary, full, work, stdin=stdin)
     assert GREP in log
     assert log.count(GREP) == 8                                     # the capture's eight ID3 messages
-    ctl = control_binary()
-    if ctl is not None:
-        assert info_lines(log) == info_lines(run_cli(ctl, full, work, stdin=stdin))
+    assert info_lines(log) == control("full_stdin" if stdin else "full_file")
