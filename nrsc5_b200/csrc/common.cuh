@@ -233,44 +233,41 @@ __device__ __forceinline__ void l2_enqueue(StreamState &st, int l2_on, unsigned 
     st.l2_nbits[e] = nbits;
 }
 
-// cu8 byte of absolute input sample n (component c); before the stream start
-// the decimator window holds zeros, i.e. byte 127 (reference src/firdecim_q15.c:33)
-__device__ __forceinline__ int q15_of_u8(int v) { return (v - 127) * 64; }
-
-// halfband decimator output y[d] for one stream (reference src/firdecim_q15.c:137-151,
-// taps int16{-134,1078,-4417,19864}): exact integer arithmetic.
-__device__ __forceinline__ short2 halfband_at(const uint8_t *iq, long long d)
+// The halfband decimator /2 of the cu8 front end (reference src/firdecim_q15.c:137-151, input.c:52-94; taps
+// int16{-134,1078,-4417,19864}) over a run of R consecutive outputs: y[r] from the cu8 words w[r] .. w[r+7], where
+// word q holds input samples 2q (low half) and 2q+1 (high half) - before the stream's first sample the words are
+// 0x7f7f7f7f, the decimator's zero history (firdecim_q15.c:33).
+//   y = x[2d-7] + sum_k ((x[2d-14+2k] + x[2d-2k]) * tap_k) >> 15,   x = (u8 - 127) * 64
+// i.e. per term (s * tap_k) >> 9 with s = u8 + u8 - 254, floored term by term as the reference does, plus 64 times the
+// centre sample.  |y| <= 256 * 25493 / 512 + 8192 < 32767: int accumulators are exact and never wrap.
+// The window slides one word per output, so each word is loaded and its bytes extracted once, not once per output
+// that uses it; the pair sums and products stay per output.  w[] and y[] may be shared or global memory.
+template <int R>
+__device__ __forceinline__ void halfband_run(const uint32_t *w, short2 *y)
 {
-    // y[d] = x[2d-7] + sum_k ((x[2d-14+2k] + x[2d-2k]) * tap_k) >> 15
     const int tap[4] = { -134, 1078, -4417, 19864 };
-    long long n0 = 2 * d - 14;
-    int accr = 0, acci = 0;
-    if (n0 >= 0) {
-        // input samples may land (asynchronous copies) while a kernel runs: read them through L2 only
-        const uint8_t *b = iq + 2 * n0;
-        auto ld = [&](int i) -> int { return q15_of_u8(__ldcg(b + i)); };
+    int lr[R + 7], li[R + 7];                     // low half of word q: the real and imaginary byte of sample 2q
+    int cr[R], ci[R];                             // high half of word r + 3: the centre sample of output r
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-            int ar = ld(4 * k) + ld(2 * (14 - 2 * k));
-            int ai = ld(4 * k + 1) + ld(2 * (14 - 2 * k) + 1);
-            accr = (short)(accr + ((ar * tap[k]) >> 15));
-            acci = (short)(acci + ((ai * tap[k]) >> 15));
+    for (int q = 0; q < R + 7; q++) {
+        const uint32_t v = w[q];
+        lr[q] = (int)(v & 0xffu);
+        li[q] = (int)((v >> 8) & 0xffu);
+        if (q >= 3 && q < R + 3) {
+            cr[q - 3] = (int)((v >> 16) & 0xffu);
+            ci[q - 3] = (int)(v >> 24);
         }
-        accr = (short)(accr + ld(14));
-        acci = (short)(acci + ld(15));
-    } else {
-        auto rd = [&](long long n, int c) -> int { return n < 0 ? 0 : q15_of_u8(__ldcg(iq + 2 * n + c)); };
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            int ar = rd(n0 + 2 * k, 0) + rd(n0 + 14 - 2 * k, 0);
-            int ai = rd(n0 + 2 * k, 1) + rd(n0 + 14 - 2 * k, 1);
-            accr = (short)(accr + ((ar * tap[k]) >> 15));
-            acci = (short)(acci + ((ai * tap[k]) >> 15));
-        }
-        accr = (short)(accr + rd(n0 + 7, 0));
-        acci = (short)(acci + rd(n0 + 7, 1));
     }
-    return make_short2((short)accr, (short)acci);
+#pragma unroll
+    for (int r = 0; r < R; r++) {
+        int ar = cr[r] * 64 - 127 * 64, ai = ci[r] * 64 - 127 * 64;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            ar += ((lr[r + k] + lr[r + 7 - k]) * tap[k] - 254 * tap[k]) >> 9;
+            ai += ((li[r + k] + li[r + 7 - k]) * tap[k] - 254 * tap[k]) >> 9;
+        }
+        y[r] = make_short2((short)ar, (short)ai);
+    }
 }
 
 }  // namespace nb

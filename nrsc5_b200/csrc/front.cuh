@@ -77,12 +77,16 @@ __device__ void set_state(const DevPtrs &p, const EngineDims &d, int s, int ns)
 // ---------------------------------------------------------------------------
 // shared memory: one buffer, reinterpreted per task phase
 // ---------------------------------------------------------------------------
+constexpr int DEMOD_RUN = 17;                      // decimated samples per thread and symbol: consecutive, a stride coprime with the 32 banks
+constexpr int TEAM_SMEM = IN_STRIDE + NSYM * (int)sizeof(short2);   // 17 344 bytes
 struct DemodSmem {
-    // per team: the FFT exchange buffer; the symbol's staged cu8 (IN_STRIDE bytes) aliases its start
-    float2 buf[TEAMS][FFT_SMEM_ELEMS];
+    // per team: the symbol's staged cu8 (IN_STRIDE bytes), then its NSYM decimated samples (short2); the FFT exchange
+    // buffer aliases the start of both
+    float2 buf[TEAMS][TEAM_SMEM / sizeof(float2)];
     float2 symphase[TEAMS];
 };
-static_assert(IN_STRIDE <= FFT_SMEM_ELEMS * sizeof(float2), "staged input must fit in the FFT buffer");
+static_assert(FFT_SMEM_ELEMS * sizeof(float2) <= TEAM_SMEM && TEAM_SMEM % 16 == 0, "a team's FFT buffer");
+static_assert(DEMOD_RUN * FFT_THREADS >= NSYM && DEMOD_RUN % 2 == 1, "a symbol's runs");
 struct PrepSmem {
     uint32_t words[ACQ_TILE + 40];                 // cu8 of one acquisition tile (+ 7 words of halfband, 31 of FIR history)
     short2 ytile[ACQ_TILE + 32];                   // its halfband outputs, preceded by the 31 the band-pass looks back on
@@ -210,24 +214,26 @@ __device__ void front_pids_flush(const DevPtrs &p, const EngineDims &d, int s, P
 // ---------------------------------------------------------------------------
 // prep (reference src/acquire.c:98-168, src/sync.c:769-777, src/firdecim_q15.c:95-109,154-158)
 // ---------------------------------------------------------------------------
-// Halfband decimator output (reference src/firdecim_q15.c:137-151, taps int16{-134,1078,-4417,19864}) from the
-// eight 32-bit words that hold its 15 input samples: word q = cu8 samples 2q (low half) and 2q+1 (high half).
-// Exact integer arithmetic: ((64*s) * tap) >> 15 == (s * tap) >> 9.
-__device__ __forceinline__ int2 halfband_words(const uint32_t *w)
+// The decimated input of one acquisition tile: ytile[k] = y[i0 - 31 + k], k < L + 31, from the tile's words in sm.words
+// (word v holds input samples 2 (start + i0 - 38 + v) and the next).  The window's first tile starts with the previous
+// window's last 31 outputs (bp_hist).  cu8: halfband_run over runs of ACQ_RUN outputs per thread; the last run is moved
+// back to end at the tile's end and overlaps its neighbour's, writing the same values.
+constexpr int ACQ_RUN = 5;                         // odd: conflict-free; 1024 runs cover ACQ_TILE + 31 outputs
+static_assert(ACQ_RUN * FRONT_THREADS >= ACQ_TILE + 31, "a tile's runs");
+__device__ __forceinline__ void acq_tile_input(const EngineDims &d, PrepSmem &sm, const StreamState &st, int i0, int L, int t)
 {
-    const int tap[4] = { -134, 1078, -4417, 19864 };
-    int ar = 0, ai = 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        const uint32_t a = w[k], b = w[7 - k];
-        const int sr = (int)(a & 0xff) + (int)(b & 0xff) - 254;
-        const int si = (int)((a >> 8) & 0xff) + (int)((b >> 8) & 0xff) - 254;
-        ar += (sr * tap[k]) >> 9;
-        ai += (si * tap[k]) >> 9;
+    const int kb = i0 == 0 ? 31 : 0;
+    if (t < kb) sm.ytile[t] = make_short2(st.bp_hist[t][0], st.bp_hist[t][1]);
+    const int n = L + 31 - kb;
+    if (d.cs16) {                                  // already decimated: the sample itself
+        for (int k = kb + t; k < L + 31; k += FRONT_THREADS) {
+            const uint32_t w = sm.words[k + 7];
+            sm.ytile[k] = make_short2((short)(w & 0xffff), (short)(w >> 16));
+        }
+    } else if (ACQ_RUN * t < n) {
+        const int k = kb + min(ACQ_RUN * t, n - ACQ_RUN);
+        halfband_run<ACQ_RUN>(sm.words + k, sm.ytile + k);
     }
-    ar += ((int)((w[3] >> 16) & 0xff) - 127) * 64;
-    ai += ((int)(w[3] >> 24) - 127) * 64;
-    return make_int2(ar, ai);
 }
 
 // NCO of a block in closed form, with the pulse shape folded in (acquire.c:243-252): nco[j] = shape[j] * exp(j*theta*j)
@@ -300,17 +306,7 @@ __device__ void front_acq_tiles(const DevPtrs &p, const EngineDims &d, int s, Pr
             sm.words[v] = a >= 0 ? __ldcg(iqw + a) : (d.cs16 ? 0u : 0x7f7f7f7fu);
         }
         __syncthreads();
-        for (int k = t; k < L + 31; k += FRONT_THREADS) {
-            if (i0 == 0 && k < 31) {                          // history: the last 31 outputs of the previous window
-                sm.ytile[k] = make_short2(st.bp_hist[k][0], st.bp_hist[k][1]);
-            } else if (d.cs16) {                              // already decimated: the sample itself
-                const uint32_t w = sm.words[k + 7];
-                sm.ytile[k] = make_short2((short)(w & 0xffff), (short)(w >> 16));
-            } else {
-                const int2 h = halfband_words(sm.words + k);
-                sm.ytile[k] = make_short2((short)h.x, (short)h.y);
-            }
-        }
+        acq_tile_input(d, sm, st, i0, L, t);
         __syncthreads();
         for (int j = t; j < L; j += FRONT_THREADS) {
             const short2 *yy = sm.ytile + j;                  // yy[k] = y[i - 31 + k]
@@ -513,17 +509,7 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
                 sm.words[v] = a >= 0 ? __ldcg(iqw + a) : (d.cs16 ? 0u : 0x7f7f7f7fu);
             }
             __syncthreads();
-            for (int k = t; k < L + 31; k += FRONT_THREADS) {
-                if (i0 == 0 && k < 31) {                          // history: the last 31 outputs of the previous window
-                    sm.ytile[k] = make_short2(st.bp_hist[k][0], st.bp_hist[k][1]);
-                } else if (d.cs16) {                              // already decimated: the sample itself
-                    const uint32_t w = sm.words[k + 7];
-                    sm.ytile[k] = make_short2((short)(w & 0xffff), (short)(w >> 16));
-                } else {
-                    const int2 h = halfband_words(sm.words + k);
-                    sm.ytile[k] = make_short2((short)h.x, (short)h.y);
-                }
-            }
+            acq_tile_input(d, sm, st, i0, L, t);
             __syncthreads();
             for (int j = t; j < L; j += FRONT_THREADS) {
                 const short2 *yy = sm.ytile + j;                  // yy[k] = y[i - 31 + k]
@@ -654,21 +640,10 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
 // ---------------------------------------------------------------------------
 // demod: one OFDM symbol per 128-thread half of the CTA
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ float2 sample_at(const uint32_t *sw, int j)
+__device__ __forceinline__ float2 sample_q15(short2 h)
 {
-    // sw points at the 32-bit word holding input samples (2*base-14, 2*base-13): output j uses words j..j+7
-    uint32_t w[8];
-#pragma unroll
-    for (int q = 0; q < 8; q++) w[q] = sw[j + q];
-    const int2 h = halfband_words(w);
     const float sc = 1.0f / 32767.0f;
     return make_float2((float)h.x * sc, (float)h.y * -sc);    // conj(x)/32767, acquire.c:160-161
-}
-
-__device__ __forceinline__ float2 sample_cs16(uint32_t w)
-{
-    const float sc = 1.0f / 32767.0f;
-    return make_float2((float)(short)(w & 0xffff) * sc, (float)(short)(w >> 16) * -sc);   // conj(x)/32767
 }
 
 __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sym, DemodSmem &sm, const float2 *nco,
@@ -710,35 +685,38 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
         sm.symphase[half] = cmul(phase0, make_float2((float)cs, (float)sn));
     }
     bar_sync(bar);
-    const float2 sp = sm.symphase[half];
 
-    // rotate by the block's NCO table (window folded in); j = n1*128 + tl
+    // sw points at the 32-bit word holding input samples (2*base-14, 2*base-13): decimated sample j uses words j..j+7
     const uint32_t *sw = reinterpret_cast<const uint32_t *>(in + off);
-    float2 v[16];
+    const short2 *y;
     if (d.cs16) {                                         // cs16 input: word j+7 is sample j of the symbol
-#pragma unroll
-        for (int n1 = 0; n1 < 16; n1++) {
-            const int j = n1 * 128 + tl;
-            v[n1] = cmul(sample_cs16(sw[j + 7]), nco[j]);
-        }
-        if (tl < NCP) {
-            const int j = NFFT + tl;
-            v[0] = cadd(v[0], cmul(sample_cs16(sw[j + 7]), nco[j]));
-        }
+        y = reinterpret_cast<const short2 *>(sw + 7);
     } else {
-#pragma unroll
-        for (int n1 = 0; n1 < 16; n1++) {
-            const int j = n1 * 128 + tl;
-            v[n1] = cmul(sample_at(sw, j), nco[j]);
-        }
-        if (tl < NCP) {                                   // fold the windowed tail onto the head (acquire.c:247-248)
-            const int j = NFFT + tl;
-            v[0] = cadd(v[0], cmul(sample_at(sw, j), nco[j]));
-        }
+        // the halfband, DEMOD_RUN consecutive samples per thread into the team's sample array (the last run is moved
+        // back to end at the symbol's last sample: it overlaps its neighbour's and writes the same values)
+        short2 *yw = reinterpret_cast<short2 *>(in + IN_STRIDE);
+        const int j0 = min(DEMOD_RUN * tl, NSYM - DEMOD_RUN);
+        halfband_run<DEMOD_RUN>(sw + j0, yw + j0);
+        y = yw;
+        bar_sync(bar);
     }
-    bar_sync(bar);                                        // every thread is done with the staged input
+    // rotate by the block's NCO table (window folded in); j = n1*128 + tl.  (Point 0 and its fold first: with all 16
+    // points' loads in flight before the fold, the 64 registers do not suffice and the FFT spills.)
+    float2 v[16];
+    v[0] = cmul(sample_q15(y[tl]), nco[tl]);
+    if (tl < NCP) {                                       // fold the windowed tail onto the head (acquire.c:247-248)
+        const int j = NFFT + tl;
+        v[0] = cadd(v[0], cmul(sample_q15(y[j]), nco[j]));
+    }
+#pragma unroll
+    for (int n1 = 1; n1 < 16; n1++) {
+        const int j = n1 * 128 + tl;
+        v[n1] = cmul(sample_q15(y[j]), nco[j]);
+    }
+    bar_sync(bar);                                        // every thread is done with the staged input and the samples
     float2 out[2][8];
     fft2048_block<true>(v, out, buf, tw, tl, bar);
+    const float2 sp = sm.symphase[half];                 // (rewritten behind the next symbol's first barrier)
 
     // kept bins (sync.c:785-789, fftshift defines.h:123-138): with q = tl + 128 h and natural bin k = q + 256 k3,
     //   k3 = 5 (q >= 222) -> compact q - 222,  k3 = 6 (q <= 232) -> q + 34      (lower sideband, bins 478..744)

@@ -29,17 +29,31 @@ void launch_fft_test(const float2 *in, float2 *out, const float2 *twid, int nfft
     k_fft_test<<<nffts, FFT_THREADS, 0, stream>>>(in, out, twid);
 }
 
-__global__ void k_halfband_test(const uint8_t *cu8, long long npairs, short2 *out)
+// the cu8 decimator alone, from a zero history: the demodulator's halfband_run (runs of 17 per thread, input words
+// staged in shared memory) over npairs outputs, i.e. 4 * npairs input bytes
+constexpr int HB_RUN = 17, HB_THREADS = 128, HB_OUT = HB_RUN * HB_THREADS;
+
+__global__ void __launch_bounds__(HB_THREADS) k_halfband_test(const uint8_t *cu8, long long npairs, short2 *out)
 {
-    long long dd = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (dd < npairs) out[dd] = halfband_at(cu8, dd);
+    __shared__ uint32_t words[HB_OUT + 7];
+    __shared__ short2 y[HB_OUT];
+    const int t = threadIdx.x;
+    const long long d0 = (long long)blockIdx.x * HB_OUT;
+    const uint32_t *cw = reinterpret_cast<const uint32_t *>(cu8);
+    for (int v = t; v < HB_OUT + 7; v += HB_THREADS) {
+        const long long q = d0 - 7 + v;                  // output d reads words d-7 .. d
+        words[v] = q >= 0 && q < npairs ? cw[q] : 0x7f7f7f7fu;
+    }
+    __syncthreads();
+    halfband_run<HB_RUN>(words + HB_RUN * t, y + HB_RUN * t);
+    __syncthreads();
+    for (int v = t; v < HB_OUT && d0 + v < npairs; v += HB_THREADS) out[d0 + v] = y[v];
 }
 
 void launch_halfband_test(const uint8_t *cu8, long long npairs, short2 *out, cudaStream_t stream)
 {
-    int th = 256;
-    long long bl = (npairs + th - 1) / th;
-    k_halfband_test<<<(unsigned)bl, th, 0, stream>>>(cu8, npairs, out);
+    const long long bl = (npairs + HB_OUT - 1) / HB_OUT;
+    if (bl > 0) k_halfband_test<<<(unsigned)bl, HB_THREADS, 0, stream>>>(cu8, npairs, out);
 }
 
 }  // namespace nb
