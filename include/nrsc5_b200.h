@@ -259,7 +259,16 @@ int nrsc5b_fft2048(int device, const float *in, float *out, int nffts);
  *     acc = sum_{u<256} W_k[u] * (x[32 n + u] - (127 + 127j));   v = (acc + 2^12) >> 13;
  *     y[k][n] = saturate16((v * conj(P[(1600 m_k n) mod 11907]) + 2^14) >> 15)
  * with the 16-bit taps W_k and the phasor table P as returned by nrsc5b_chan_tables.  Runs on the tensor cores
- * (wgmma u8 x s8, TMA-fed, accumulators in registers). */
+ * (wgmma u8 x s8, TMA-fed, accumulators in registers).
+ *
+ * Streaming (nrsc5b_chan_push, nrsc5b_chan_feed): a live capture arrives in pieces, so a handle keeps two values,
+ *     T, the complex samples pushed since create / nrsc5b_chan_reset, and the carry, the last < 256 samples it has not
+ *     consumed yet.
+ * With N(T) = T >= 256 ? (T - 256) / 32 + 1 : 0, a push that takes T to T' emits exactly outputs N(T) .. N(T') - 1 of
+ * every channel, n in the mixer's phasor index being that absolute output index; the carry kept afterwards is the
+ * samples from 32 N(T') on (at most 255 samples, 510 bytes).  So pushing a capture in pieces of any even byte count
+ * (shorter than the filter, not a multiple of 64, empty) gives, concatenated, the outputs of nrsc5b_chan_run on the
+ * whole capture, bit for bit.  The one-shot entry points (nrsc5b_chan_run*) neither use nor change T and the carry. */
 typedef struct nrsc5b_channelizer nrsc5b_channelizer_t;
 int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch);
 void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c);
@@ -274,6 +283,26 @@ long long nrsc5b_chan_outputs(size_t nbytes);
 int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8, size_t nbytes, void *d_out, size_t out_stride, void *cuda_stream);
 /* host capture -> host out[nch][2 * outputs]; synchronous (tests) */
 int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, int16_t *out);
+/* Start the stream over: T = 0, the carry is dropped. */
+int nrsc5b_chan_reset(nrsc5b_channelizer_t *c);
+/* Push the next nbytes (even; otherwise NRSC5B_EINVAL) of the capture and write the outputs they complete to the
+ * device buffer d_out[nch][out_stride] (int16 values, I/Q interleaved; row k = channel k, this push's first output at
+ * column 0; out_stride even and >= 2 * *nout, d_out 4-byte aligned).  cu8 may be pageable or page-locked host memory or
+ * device memory.  Asynchronous on cuda_stream (a cudaStream_t cast to void*, NULL = default); page-locked and device
+ * input must stay valid until the stream has run the copy.  *nout (may be NULL) = outputs written per channel,
+ * N(T') - N(T).  Internally the channeliser stages up to 4 MiB at a time, so a push of any size works. */
+int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, void *d_out, size_t out_stride, void *cuda_stream,
+                     long long *nout);
+/* The same push, but channel k is appended straight to the input of stream streams[k] of the cs16 engine `e` (streams
+ * NULL: stream k), as nrsc5b_push_cs16 would append it.  `e` must be an FM engine created with input_cs16 = 1 on the
+ * channeliser's device that reads its own input buffers (not nrsc5b_attach_device_input); the stream indices must be
+ * distinct and < nstreams.  Otherwise, and for odd nbytes: NRSC5B_EINVAL, nothing changed.
+ * Runs on the engine's CUDA stream and publishes each stream's new sample count after the kernel; it does not wait for
+ * the GPU, except for the synchronous trim a full stream gets (as in nrsc5b_push_cs16).  All or nothing: if a target
+ * stream has no room for the push's outputs even after trimming, it returns NRSC5B_EFULL and neither the channeliser
+ * nor the engine has taken any of it - run nrsc5b_process and push the same bytes again.  Like nrsc5b_process, it must
+ * not be mixed with an asynchronous batch in flight (nrsc5b_submit .. nrsc5b_poll). */
+int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const uint8_t *cu8, size_t nbytes);
 
 const char *nrsc5b_version(void);
 

@@ -26,8 +26,19 @@ def _lib():
         L.nrsc5b_chan_outputs.restype = ctypes.c_longlong
         L.nrsc5b_chan_run_device.argtypes = [vp, vp, sz, vp, sz, vp]
         L.nrsc5b_chan_run.argtypes = [vp, vp, sz, vp]
+        L.nrsc5b_chan_reset.argtypes = [vp]
+        L.nrsc5b_chan_push.argtypes = [vp, vp, sz, vp, sz, vp, ctypes.POINTER(ctypes.c_longlong)]
+        L.nrsc5b_chan_feed.argtypes = [vp, vp, vp, vp, sz]
         L._chan_ready = True
     return L
+
+
+def stream_outputs(pushed: int, nbytes: int) -> int:
+    """Outputs per channel a push of nbytes emits after `pushed` complex samples (include/nrsc5_b200.h):
+    N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0."""
+    def n(t):
+        return (t - TAPS) // DECIM + 1 if t >= TAPS else 0
+    return n(pushed + nbytes // 2) - n(pushed)
 
 
 def make_tables(offsets_100khz):
@@ -50,6 +61,8 @@ class Channelizer:
         self.nch = int(self.offsets.size)
         self._h = ctypes.c_void_p()
         _check(self._L.nrsc5b_chan_create(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), "nrsc5b_chan_create")
+        self.device = device
+        self.pushed = 0                 # T: complex samples pushed since create / reset (mirrors the handle's count)
 
     def close(self):
         if self._h:
@@ -86,3 +99,50 @@ class Channelizer:
     def run_device(self, d_cu8: int, nbytes: int, d_out: int, out_stride: int, stream: int = 0):
         _check(self._L.nrsc5b_chan_run_device(self._h, ctypes.c_void_p(d_cu8), nbytes, ctypes.c_void_p(d_out), out_stride,
                                              ctypes.c_void_p(stream)), "nrsc5b_chan_run_device")
+
+    # ---- streaming: a capture pushed in pieces; the outputs concatenate to run() of the whole capture ----
+    def reset(self):
+        _check(self._L.nrsc5b_chan_reset(self._h), "nrsc5b_chan_reset")
+        self.pushed = 0
+
+    def push_device(self, ptr: int, nbytes: int, d_out: int, out_stride: int, stream: int = 0) -> int:
+        """The next nbytes of the capture at ptr (host or device memory) -> the outputs they complete, written to the
+        device buffer d_out[nch][out_stride] (int16 values); asynchronous on `stream`.  Returns the outputs per channel."""
+        n = ctypes.c_longlong(0)
+        _check(self._L.nrsc5b_chan_push(self._h, ctypes.c_void_p(ptr), nbytes, ctypes.c_void_p(d_out), out_stride,
+                                        ctypes.c_void_p(stream), ctypes.byref(n)), "nrsc5b_chan_push")
+        self.pushed += nbytes // 2
+        return int(n.value)
+
+    def push(self, cu8: np.ndarray) -> np.ndarray:
+        """The next piece of the capture (uint8, I/Q interleaved, even length) -> int16 [nch][2 * n]: the outputs it
+        completes.  Synchronous."""
+        import torch
+        a = np.ascontiguousarray(cu8, dtype=np.uint8).reshape(-1)
+        n = stream_outputs(self.pushed, a.size)
+        dev = torch.device("cuda", self.device)
+        out = torch.empty((self.nch, 2 * max(n, 1)), dtype=torch.int16, device=dev)
+        stream = torch.cuda.current_stream(dev)
+        got = self.push_device(a.ctypes.data if a.size else 0, a.size, out.data_ptr(), out.shape[1], stream.cuda_stream)
+        assert got == n
+        stream.synchronize()
+        return out[:, : 2 * n].cpu().numpy()
+
+    def feed(self, engine, data, streams=None):
+        """The next piece of the capture -> channel k appended to cs16 stream streams[k] of `engine` (an Engine made
+        with input_cs16=True; streams None: stream k).  data: a uint8 numpy array or (pointer, nbytes) to host or device
+        memory.  Raises EngineError on NRSC5B_EFULL (nothing taken: process() and feed the same data again)."""
+        if isinstance(data, tuple):
+            ptr, nbytes = int(data[0]), int(data[1])
+            keep = None
+        else:
+            keep = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+            ptr, nbytes = (keep.ctypes.data if keep.size else 0), keep.size
+        st = None
+        if streams is not None:
+            st = np.ascontiguousarray(streams, dtype=np.int32)
+            if st.size != self.nch:
+                raise ValueError(f"streams: {st.size} entries for {self.nch} channels")
+        _check(self._L.nrsc5b_chan_feed(self._h, engine._h, None if st is None else st.ctypes.data, ctypes.c_void_p(ptr),
+                                        nbytes), "nrsc5b_chan_feed")
+        self.pushed += nbytes // 2

@@ -40,6 +40,7 @@
 #include <vector>
 
 #include "../../include/nrsc5_b200.h"
+#include "chan_feed.h"
 
 namespace nbch {
 
@@ -55,17 +56,20 @@ constexpr int STAGES = 4;
 constexpr uint32_t A_STAGE_BYTES = NCHUNK * TILE_M * CHUNK;      // 32768
 constexpr uint32_t W_BYTES = NCHUNK * TILE_N * CHUNK;            // 65536
 constexpr int HALF = PERIOD / 2 + 1;                              // phasor table entries 0 .. 5953; the rest are their conjugates
-constexpr uint32_t EPI_BYTES = ((HALF * 4 + 15) & ~15) + GROUP * 4 + 2 * GROUP * 4;   // half table, rotation steps, offset corrections
+// half table, rotation steps, offset corrections, destination offsets
+constexpr uint32_t EPI_BYTES = ((HALF * 4 + 15) & ~15) + GROUP * 4 + 2 * GROUP * 4 + GROUP * 8;
 constexpr uint32_t SMEM_BYTES = W_BYTES + STAGES * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
 static_assert(SMEM_BYTES <= 227 * 1024, "more shared memory than an H100 block may have");
 
 struct Params {
     int nch;                   // channels
     int ngroups;
+    int n0mod;                 // (absolute index of this launch's output 0) mod 11907: the mixer runs on across launches
     long long nout;            // output samples per channel
     long long tiles;           // ceil(nout / TILE_M)
-    int16_t *out;              // [nch][out_stride] cs16 (I, Q interleaved): int16 pairs
-    size_t out_stride;         // int16 values between channels
+    int16_t *out;              // cs16 (I, Q interleaved): output n of channel k goes to out + dst[k] + 2 n
+    const long long *dst;      // [nch] int16 offsets of each channel's output 0; null: dst[k] = k * out_stride
+    size_t out_stride;
     const int *rot_step;       // [nch] (1600 m_k) mod 11907
     const long long *corr;     // [nch][2] 127 * (sum Wr - sum Wi), 127 * (sum Wi + sum Wr)   (already in acc units)
     const short2 *phasor;      // [PERIOD]
@@ -151,10 +155,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     uint8_t *smem_a = smem + W_BYTES;                              // [STAGES][8 chunks][64 rows][64 B]
     Barriers &bar = *reinterpret_cast<Barriers *>(smem + W_BYTES + STAGES * A_STAGE_BYTES);
     // the epilogue's tables in shared memory: the first half of the phasor table (P[11907 - i] = conj(P[i]), made so on
-    // the host), and this group's rotation steps and offset corrections
+    // the host), and this group's rotation steps, offset corrections and output destinations
     short2 *ph_half = reinterpret_cast<short2 *>(smem + W_BYTES + STAGES * A_STAGE_BYTES + 256);
     int *s_rot = reinterpret_cast<int *>(reinterpret_cast<uint8_t *>(ph_half) + ((HALF * 4 + 15) & ~15));
     uint32_t *s_corr = reinterpret_cast<uint32_t *>(s_rot + GROUP);
+    long long *s_dst = reinterpret_cast<long long *>(s_corr + 2 * GROUP);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int group = (int)blockIdx.x % p.ngroups, slot = (int)blockIdx.x / p.ngroups, nslots = (int)gridDim.x / p.ngroups;
 
@@ -164,6 +169,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
         s_rot[i] = p.rot_step[ch];
         s_corr[2 * i] = (uint32_t)p.corr[2 * ch];
         s_corr[2 * i + 1] = (uint32_t)p.corr[2 * ch + 1];
+        s_dst[i] = p.dst ? p.dst[ch] : (long long)ch * (long long)p.out_stride;
     }
     if (threadIdx.x == 0) {
         mbar_init(&bar.w_full, 1);
@@ -197,6 +203,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     // ===== consumers: warpgroup 1 takes the CTA's even tiles, warpgroup 2 the odd ones =====
     const int wg = wgi - 1, wwarp = warp & 3;
     const int q = lane & 3;                                        // this thread's channels: cl = 4 i + q, i = 0 .. 7
+    int16_t *row[8];                                               // where their output 0 goes
+#pragma unroll
+    for (int i = 0; i < 8; i++) row[i] = p.out + s_dst[4 * i + q];
     mbar_wait(&bar.w_full, 0);
     unsigned it = (unsigned)wg;
     for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2) {
@@ -220,11 +229,13 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
         // ===== epilogue: rows 16 wwarp + lane / 4 (h = 0) and + 8 (h = 1) of the tile =====
         // 32-bit arithmetic throughout: 256 * hi + lo wraps, the filter output itself is bounded by
         // 128 * sum(|Wr| + |Wi|) < 2^28 (checked when the tables are made), so the wrapped sum is the value; after
-        // the shift a component is below 2^15 and the rotation's two products stay below 2^31.
+        // the shift a component is below 2^15 and the rotation's two products stay below 2^31.  The phasor index
+        // (1600 m_k (n0 + n)) mod 11907 is taken from nmod = (n0 mod 11907 + n) mod 11907 < 11907, so its product
+        // with the rotation step stays below 11907^2 < 2^32.
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             const long long n = tile * TILE_M + 16 * wwarp + (lane >> 2) + 8 * h;
-            const int nmod = (int)(n % PERIOD);
+            const int nmod = (int)((p.n0mod + n) % PERIOD);
 #pragma unroll
             for (int i = 0; i < 8; i++) {
                 const int cl = 4 * i + q, ch = group * GROUP + cl;
@@ -241,11 +252,26 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
                 zr = zr > 32767 ? 32767 : (zr < -32768 ? -32768 : zr);
                 zi = zi > 32767 ? 32767 : (zi < -32768 ? -32768 : zi);
                 const uint32_t packed = (uint32_t)(uint16_t)(int16_t)zr | ((uint32_t)(uint16_t)(int16_t)zi << 16);
-                if (ch < p.nch && n < p.nout) *reinterpret_cast<uint32_t *>(p.out + (size_t)ch * p.out_stride + 2 * n) = packed;
+                if (ch < p.nch && n < p.nout) *reinterpret_cast<uint32_t *>(row[i] + 2 * n) = packed;
             }
         }
     }
 }
+
+// Streaming: after a launch over the staging buffer has used the outputs it could, the samples from 32 x (outputs) on -
+// at most 255 samples - move to the front of the buffer, where the next push's bytes are appended to them.  Source and
+// destination can overlap: one block reads everything before it writes.
+__global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
+{
+    const int i = 2 * (int)threadIdx.x;
+    uint16_t v = 0;
+    if (i < nbytes) v = *reinterpret_cast<const uint16_t *>(buf + from + i);
+    __syncthreads();
+    if (i < nbytes) *reinterpret_cast<uint16_t *>(buf + i) = v;
+}
+
+constexpr size_t STAGE_CAP = (4u << 20) + 512;                    // staging: the carry (< 512 bytes) + 4 MiB of new capture
+constexpr int DST_RING = 8;                                       // destination tables in flight (nrsc5b_chan_feed)
 
 }  // namespace nbch
 
@@ -265,6 +291,14 @@ struct nrsc5b_channelizer {
     short2 *d_phasor;
     CUtensorMap map_w;
     PFN_cuTensorMapEncodeTiled_v12000 encode;
+    // streaming (nrsc5b_chan_push / nrsc5b_chan_feed)
+    long long pushed;                     // T: complex samples pushed since create / reset
+    uint8_t *d_stage;                     // [STAGE_CAP]: carry (samples from 32 N(T) on) | the bytes being pushed
+    CUtensorMap map_stage;
+    cudaEvent_t stage_done;               // the last work that used d_stage (pushes may come on different CUDA streams)
+    long long *h_dst, *d_dst;             // [DST_RING][nch] page-locked / device: per-channel destinations of a feed
+    cudaEvent_t dst_copied[DST_RING];
+    unsigned dst_pos;
 };
 
 static double bessel_i0(double x)
@@ -375,6 +409,9 @@ extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const 
     c->ngroups = (nch + GROUP - 1) / GROUP;
     c->offsets.assign(offsets_100khz, offsets_100khz + nch);
     c->d_w = nullptr; c->d_rot = nullptr; c->d_corr = nullptr; c->d_phasor = nullptr;
+    c->pushed = 0; c->d_stage = nullptr; c->stage_done = nullptr;
+    c->h_dst = nullptr; c->d_dst = nullptr; c->dst_pos = 0;
+    for (int i = 0; i < DST_RING; i++) c->dst_copied[i] = nullptr;
     // driver entry point for the tensor-map encoder (no link-time dependency on libcuda)
     {
         void *fn = nullptr;
@@ -401,6 +438,17 @@ extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const 
         ok = c->encode(&c->map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_w, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                        CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
+    // the streaming staging buffer as a [rows][64 B] capture matrix (rows past a launch's valid bytes only feed outputs
+    // the launch does not write)
+    ok = ok && cudaMalloc(&c->d_stage, STAGE_CAP) == cudaSuccess && cudaMemset(c->d_stage, 0, STAGE_CAP) == cudaSuccess &&
+         cudaEventCreateWithFlags(&c->stage_done, cudaEventDisableTiming) == cudaSuccess;
+    if (ok) {
+        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)(STAGE_CAP / CHUNK) };
+        const cuuint64_t strides[1] = { CHUNK };
+        const cuuint32_t box[2] = { CHUNK, TILE_M }, es[2] = { 1, 1 };
+        ok = c->encode(&c->map_stage, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_stage, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    }
     if (ok) ok = cudaFuncSetAttribute(k_channelize, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) == cudaSuccess;
     if (!ok) {
         nrsc5b_chan_destroy(c);
@@ -417,6 +465,12 @@ extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
     cudaFree(c->d_rot);
     cudaFree(c->d_corr);
     cudaFree(c->d_phasor);
+    cudaFree(c->d_stage);
+    cudaFree(c->d_dst);
+    if (c->h_dst) cudaFreeHost(c->h_dst);
+    if (c->stage_done) cudaEventDestroy(c->stage_done);
+    for (int i = 0; i < DST_RING; i++)
+        if (c->dst_copied[i]) cudaEventDestroy(c->dst_copied[i]);
     delete c;
 }
 
@@ -430,11 +484,132 @@ extern "C" int nrsc5b_chan_tables(nrsc5b_channelizer_t *c, int16_t *taps, int16_
     return NRSC5B_OK;
 }
 
+// N(T): outputs whose 256-sample windows lie within the first T samples of a capture
+static long long outputs_of(long long samples) { return samples < TAPS ? 0 : (samples - TAPS) / DECIM + 1; }
+
 /* How many output samples a capture of `nbytes` gives per channel: every output needs 256 input samples. */
-extern "C" long long nrsc5b_chan_outputs(size_t nbytes)
+extern "C" long long nrsc5b_chan_outputs(size_t nbytes) { return outputs_of((long long)(nbytes / 2)); }
+
+// outputs n0 .. n0 + nout - 1 of the capture whose sample 32 n0 is row 0 of map_x: output n0 + j of channel k goes to
+// out + dst[k] + 2 j (dst null: k * out_stride)
+static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0, long long nout, int16_t *out, const long long *dst,
+                  size_t out_stride, cudaStream_t stream)
 {
-    const long long samples = (long long)(nbytes / 2);
-    return samples < TAPS ? 0 : (samples - TAPS) / DECIM + 1;
+    Params p;
+    p.nch = c->nch;
+    p.ngroups = c->ngroups;
+    p.n0mod = (int)(n0 % PERIOD);
+    p.nout = nout;
+    p.tiles = (nout + TILE_M - 1) / TILE_M;
+    p.out = out;
+    p.dst = dst;
+    p.out_stride = out_stride;
+    p.rot_step = c->d_rot;
+    p.corr = c->d_corr;
+    p.phasor = c->d_phasor;
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+    long long slots = sms / c->ngroups;
+    if (slots < 1) slots = 1;
+    if (slots > p.tiles) slots = p.tiles;
+    k_channelize<<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
+    return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+}
+
+// The streaming core of nrsc5b_chan_push and nrsc5b_chan_feed: appends nbytes (even) of capture at `src` to the
+// handle's stream and writes the outputs they complete, N(T) .. N(T') - 1, output N(T) + j of channel k to
+// out + dst[k] + 2 j (dst: a device table; null: k * out_stride).  Pushes larger than the staging buffer go through it
+// in pieces.  Asynchronous on `stream`; the source is read by a copy on that stream.
+static int stream_in(nrsc5b_channelizer *c, const uint8_t *src, size_t nbytes, int16_t *out, const long long *dst, size_t out_stride,
+                     cudaStream_t stream)
+{
+    if (!nbytes) return NRSC5B_OK;
+    // device memory: a device-to-device copy; page-locked host memory: DMA straight from it; pageable host memory: the
+    // driver stages it (the copy returns once it has read the caller's bytes)
+    cudaPointerAttributes attr;
+    const bool on_device = cudaPointerGetAttributes(&attr, src) == cudaSuccess &&
+                           (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+    cudaGetLastError();
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;
+    long long written = 0;
+    for (size_t done = 0; done < nbytes;) {
+        const long long first = outputs_of(c->pushed);            // absolute index of staging row 0's output
+        const size_t carry = 2 * (size_t)(c->pushed - DECIM * first);
+        const size_t piece = (nbytes - done < STAGE_CAP - carry ? nbytes - done : STAGE_CAP - carry) & ~(size_t)1;
+        if (cudaMemcpyAsync(c->d_stage + carry, src + done, piece, kind, stream) != cudaSuccess) return NRSC5B_ECUDA;
+        const long long held = (long long)(carry + piece) / 2, nl = outputs_of(held);
+        if (nl > 0) {
+            int rc = launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream);
+            if (rc) return rc;
+            k_move_carry<<<1, 256, 0, stream>>>(c->d_stage, (size_t)CHUNK * nl, (int)(2 * (held - DECIM * nl)));
+            if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
+        }
+        c->pushed += (long long)(piece / 2);
+        written += nl;
+        done += piece;
+    }
+    return cudaEventRecord(c->stage_done, stream) == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+}
+
+extern "C" int nrsc5b_chan_reset(nrsc5b_channelizer_t *c)
+{
+    if (!c) return NRSC5B_EINVAL;
+    c->pushed = 0;                                            // the carry is what lies beyond 32 N(T): nothing now
+    return NRSC5B_OK;
+}
+
+extern "C" int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, void *d_out, size_t out_stride,
+                                void *cuda_stream, long long *nout)
+{
+    if (nout) *nout = 0;
+    if (!c || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
+    const long long n = outputs_of(c->pushed + (long long)(nbytes / 2)) - outputs_of(c->pushed);
+    if (n > 0 && (!d_out || ((uintptr_t)d_out & 3) || (out_stride & 1) || (size_t)(2 * n) > out_stride)) return NRSC5B_EINVAL;
+    if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
+    const int rc = stream_in(c, cu8, nbytes, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride,
+                             reinterpret_cast<cudaStream_t>(cuda_stream));
+    if (rc == NRSC5B_OK && nout) *nout = n;
+    return rc;
+}
+
+extern "C" int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const uint8_t *cu8, size_t nbytes)
+{
+    if (!c || !e || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
+    const long long n = outputs_of(c->pushed + (long long)(nbytes / 2)) - outputs_of(c->pushed);
+    if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
+    const size_t nch = (size_t)c->nch;
+    if (!c->h_dst) {
+        bool ok = cudaHostAlloc(reinterpret_cast<void **>(&c->h_dst), DST_RING * nch * sizeof(long long), cudaHostAllocDefault) == cudaSuccess;
+        if (!ok) c->h_dst = nullptr;
+        ok = ok && cudaMalloc(&c->d_dst, DST_RING * nch * sizeof(long long)) == cudaSuccess;
+        for (int i = 0; ok && i < DST_RING; i++) ok = cudaEventCreateWithFlags(&c->dst_copied[i], cudaEventDisableTiming) == cudaSuccess;
+        if (!ok) {
+            if (c->h_dst) cudaFreeHost(c->h_dst);
+            cudaFree(c->d_dst);
+            for (int i = 0; i < DST_RING; i++)
+                if (c->dst_copied[i]) cudaEventDestroy(c->dst_copied[i]);
+            c->h_dst = c->d_dst = nullptr;
+            for (int i = 0; i < DST_RING; i++) c->dst_copied[i] = nullptr;
+            return NRSC5B_ENOMEM;
+        }
+    }
+    // a slot of the destination ring is rewritten DST_RING feeds after its copy was queued: by then it has long run
+    const unsigned slot = c->dst_pos % DST_RING;
+    if (cudaEventSynchronize(c->dst_copied[slot]) != cudaSuccess) return NRSC5B_ECUDA;
+    long long *h_dst = c->h_dst + slot * nch, *d_dst = c->d_dst + slot * nch;
+    FeedTarget t;
+    int rc = nbfeed_reserve(e, c->device, streams, c->nch, n, &t, h_dst);
+    if (rc) return rc;
+    if (n > 0) {
+        if (cudaMemcpyAsync(d_dst, h_dst, nch * sizeof(long long), cudaMemcpyHostToDevice, t.stream) != cudaSuccess ||
+            cudaEventRecord(c->dst_copied[slot], t.stream) != cudaSuccess)
+            return NRSC5B_ECUDA;
+        c->dst_pos++;
+    }
+    rc = stream_in(c, cu8, nbytes, t.base, d_dst, 0, t.stream);
+    if (rc) return rc;
+    return nbfeed_commit(e, streams, c->nch, n);
 }
 
 /* Device-resident capture (cu8, I/Q interleaved, 23 814 000 S/s; 64-byte aligned, nbytes of it valid) -> out[nch][out_stride]
@@ -455,23 +630,7 @@ extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8
     if (c->encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void *>(d_cu8), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
         return NRSC5B_ECUDA;
-    Params p;
-    p.nch = c->nch;
-    p.ngroups = c->ngroups;
-    p.nout = nout;
-    p.tiles = (nout + TILE_M - 1) / TILE_M;
-    p.out = reinterpret_cast<int16_t *>(d_out);
-    p.out_stride = out_stride;
-    p.rot_step = c->d_rot;
-    p.corr = c->d_corr;
-    p.phasor = c->d_phasor;
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
-    long long slots = sms / c->ngroups;
-    if (slots < 1) slots = 1;
-    if (slots > p.tiles) slots = p.tiles;
-    k_channelize<<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, reinterpret_cast<cudaStream_t>(cuda_stream)>>>(map_x, c->map_w, p);
-    return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+    return launch(c, map_x, 0, nout, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 /* Host convenience (tests): host capture in, host cs16 out[nch][2 * outputs]. */

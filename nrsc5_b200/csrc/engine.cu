@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/nrsc5_b200.h"
+#include "chan_feed.h"
 #include "common.cuh"
 // NVTX ranges around the host-side phases (header-only NVTX 3: no library to link; a no-op unless a tool is attached -
 // `ncu --nvtx`, Nsight Systems): process / submit / poll, and per pass the front end and the decode groups
@@ -1548,6 +1549,55 @@ extern "C" int nrsc5b_attach_device_input(nrsc5b_engine_t *e, const void *dev_bu
         int rc = publish_avail(e, s, e->stream);
         if (rc) return rc;
     }
+    return NRSC5B_OK;
+}
+
+// The engine's side of nrsc5b_chan_feed (chan_feed.h): the channeliser writes cs16 samples straight behind each
+// target stream's data in the engine's own input buffers, on the engine's CUDA stream.
+int nbfeed_reserve(nrsc5b_engine_t *e, int device, const int *streams, int nch, long long nout, FeedTarget *t, long long *dst)
+{
+    if (!e || !t || !dst || nch <= 0 || nout < 0) return NRSC5B_EINVAL;
+    if (e->cfg.mode != NRSC5B_MODE_FM || !e->dims.cs16 || !e->iq_owned || e->dp.iq != e->iq_owned || device != e->cfg.device ||
+        e->in_flight)
+        return NRSC5B_EINVAL;
+    const int S = e->dims.nstreams;
+    if (!streams && nch > S) return NRSC5B_EINVAL;
+    std::vector<uint8_t> seen(S, 0);
+    for (int k = 0; k < nch; k++) {
+        const int s = streams ? streams[k] : k;
+        if (s < 0 || s >= S || seen[s]) return NRSC5B_EINVAL;
+        seen[s] = 1;
+    }
+    // all or nothing: every target stream must take the whole push (trim the full ones, then look again)
+    const size_t need = 4 * (size_t)nout;
+    bool full = false;
+    for (int k = 0; k < nch; k++) {
+        const int s = streams ? streams[k] : k;
+        if ((size_t)e->pushed[s] * 2 + need <= e->dims.in_stride) continue;
+        int rc = trim_stream(e, s);
+        if (rc) return rc;
+        if ((size_t)e->pushed[s] * 2 + need > e->dims.in_stride) full = true;
+    }
+    if (full) return NRSC5B_EFULL;
+    t->stream = e->stream;
+    t->base = reinterpret_cast<int16_t *>(e->iq_owned);
+    for (int k = 0; k < nch; k++) {
+        const int s = streams ? streams[k] : k;
+        dst[k] = (long long)(((size_t)s * e->dims.in_stride + (size_t)e->pushed[s] * 2) / sizeof(int16_t));
+    }
+    return NRSC5B_OK;
+}
+
+int nbfeed_commit(nrsc5b_engine_t *e, const int *streams, int nch, long long nout)
+{
+    if (nout <= 0) return NRSC5B_OK;
+    for (int k = 0; k < nch; k++) {
+        const int s = streams ? streams[k] : k;
+        e->pushed[s] += 2 * nout;                              // 2-byte units: a cs16 sample counts as two
+        int rc = publish_avail(e, s, e->stream);               // on the feed's stream, i.e. after the samples
+        if (rc) return rc;
+    }
+    e->direct_push = true;
     return NRSC5B_OK;
 }
 
