@@ -27,12 +27,33 @@ constexpr int P1_VIT = P1_LEN * 3;          // 438528
 constexpr int P1_STEPS = P1_LEN + 64;       // tail-biting: 32 pre-roll + 32 post-roll
 constexpr int PIDS_LEN = 80;
 constexpr int P3_LEN = 4608;                // P3 frame bits in MP3/MP11 (reference src/defines.h:53)
-constexpr int P3_VIT = P3_LEN * 3;          // 13824
-constexpr int PX1_BLOCK = 4608;             // PX1 soft bits per block (2 partitions per sideband)
 constexpr int IV_N = 147456;                // span of interleaver IV (reference src/decode.c:350)
 constexpr int PX_RING = 2 * IV_N;
 constexpr int P3_SLOTS = 8;                 // P3 frames per stream and pass (one per two blocks)
 constexpr int P3_DEC_STRIDE = 5120;         // decisions per frame: 5 fallback chunks of 1024 >= 4608 + 64
+constexpr int P3S_LEN = 2304, IV_NS = IV_N / 2;    // MP2: P3 frame bits, interleaver IV span (decode.c:346-350)
+
+// The extended-partition decode groups, in launch order - the reference's call order, P3 before P4:
+//   0 = MP3 / MP11's P3, 1 = MP2's short P3, 2 = MP11's P4.
+// len: frame bits, which are also the group's soft bits per block; its interleaver IV spans 32 frames (IV_N, IV_NS)
+// and reads the delay table iv_delay (len == P3_LEN) or iv_delay_s.  ring: 0 = PX1, 1 = PX2.  lc: logical channel.
+// modes: bit m set = compatibility mode m feeds the group (a mode feeds at most one group per ring).
+// The host launches a group once a stream has asked for it: bit g of px_need_of(mode).
+struct PxGroup { int len, ring, lc, modes; };
+constexpr int PX_GROUPS = 3;
+__host__ __device__ constexpr PxGroup px_group(int g)
+{
+    return g == 0 ? PxGroup{ P3_LEN, 0, 1, 1 << 3 | 1 << 11 }
+         : g == 1 ? PxGroup{ P3S_LEN, 0, 1, 1 << 2 }
+                  : PxGroup{ P3_LEN, 1, 2, 1 << 11 };
+}
+static_assert(32 * P3_LEN == IV_N && 32 * P3S_LEN == IV_NS, "a group's interleaver IV spans 32 frames");
+__host__ __device__ constexpr int px_need_of(int cm)
+{
+    int need = 0;
+    for (int g = 0; g < PX_GROUPS; g++) need |= (px_group(g).modes >> cm & 1) << g;
+    return need;
+}
 constexpr int ST_NONE = 0, ST_COARSE = 1, ST_FINE = 2;
 
 // record types (include/nrsc5_b200.h)
@@ -85,20 +106,14 @@ struct StreamState {
     int pids_pending;          // PIDS frames (of blocks pids_bc[]) waiting to be decoded into the log slots pids_rec[];
     int pids_bc[16];           // k_stream decodes them together, one warp each, before it exits
     unsigned pids_rec[16];
-    // P3 (MP3/MP11 PX1 partitions): convolutional interleaver IV bookkeeping (reference src/decode.c:344-414)
-    long long px_total;        // PX1 soft bits taken in since the interleaver (re)started
-    int px_started;
-    int p3_pending;            // P3 frames waiting for the decode kernels that follow k_stream
-    long long p3_k0[8];        // interleaver position of each frame's first soft bit
-    unsigned p3_rec[8];        // log offset of each frame's reserved FRAME record
-    // the other extended-partition channels, decoded by kernel groups the host only launches once a stream has
-    // asked for them (g_px_need): [0] = MP2's 2304-bit P3 frames (PX1 ring, one partition per sideband),
-    // [1] = MP11's P4 frames (PX2 ring)
-    long long px2_total;       // PX2 soft bits taken in since the interleaver (re)started
-    int px2_started;
-    int xq_pending[2];
-    long long xq_k0[2][8];
-    unsigned xq_rec[2][8];
+    // extended partitions: convolutional interleaver IV bookkeeping per ring, [0] = PX1, [1] = PX2 (reference
+    // src/decode.c:344-437) ...
+    long long px_total[2];     // soft bits taken in since the interleaver (re)started
+    int px_started[2];
+    // ... and per decode group (px_group) the frames waiting for the decode kernels that follow k_stream
+    int xq_pending[PX_GROUPS];
+    long long xq_k0[PX_GROUPS][P3_SLOTS];  // interleaver position of each frame's first soft bit
+    unsigned xq_rec[PX_GROUPS][P3_SLOTS];  // log offset of each frame's reserved FRAME record
     int force_state;           // host override (nrsc5b_set_sync_state), -1 = none
     // L2 on the device (l2.cuh): what the pass handed to L2 so far, in the reference's call order - frames by the log
     // offset of their packed bits (0xffffffff: the log was full), nbits == 0 for a frame_reset (entering fine sync)
@@ -128,29 +143,27 @@ struct EngineDims {
     size_t log_cap;            // bytes of log per stream
     int emit_soft;
     int cs16;                  // input is cs16 at the decimated rate: 4 bytes per sample, no halfband
-    int px_enabled;            // PX_NEED_* bits: the extended-partition decode groups the host launches after k_stream
+    int px_enabled;            // bit g: the host launches extended-partition decode group g after k_stream
     int l2;                    // frames also go through L2 on the device (nrsc5b_enable_l2)
     int cluster;               // CTAs per stream in k_stream (thread-block cluster): 1, 2 or 4
 };
 
-// buffers of one extra extended-partition decode group (same roles as the p3_* arrays)
+// buffers of one extended-partition decode group, [S][P3_SLOTS]... (null until the host enables the group)
 struct PxBufs {
-    int8_t *vin;
-    uint2 *dec;
-    uint32_t *spec, *end;
-    int *endstate;
-    uint2 *fspec, *fend;
-    int *fhstate, *ftbend;
-    uint32_t *bits;
-    int *flags;
+    int8_t *vin;               // [3 * len] deinterleaved + depunctured soft bits
+    uint2 *dec;                // [P3_DEC_STRIDE] survivor decisions
+    uint32_t *spec, *end;      // [19][32] fast Viterbi chunk boundary metrics
+    int *endstate;             // [1]
+    uint2 *fspec, *fend;       // [5][16] fallback Viterbi
+    int *fhstate, *ftbend;     // [5]
+    uint32_t *bits;            // [len / 32] decoded (still scrambled) bits
+    int *flags;                // [4] ready, slow, retry, -
 };
-constexpr int PX_NEED_SHORT = 1, PX_NEED_PX2 = 2, PX_NEED_P3 = 4;   // MP2 | MP11 (P4) | MP3 and MP11 (4608-bit P3)
-constexpr int P3S_LEN = 2304, IV_NS = IV_N / 2;    // MP2: P3 frame bits, interleaver IV span (decode.c:346-350)
 
 // Per-engine control words in device memory (one engine = one instance: engines on one device share nothing).
 struct EngineCtl {
     unsigned long long progress;   // bumped by every stream that processed a block
-    unsigned px_need;              // PX_NEED_* bits: a stream waits for a decode group the host has not enabled
+    unsigned px_need;              // bit g: a stream waits for decode group g, which the host has not enabled
     unsigned more;                 // streams that could go on after the last pass of a batch (a full window is buffered)
 };
 
@@ -181,19 +194,10 @@ struct DevPtrs {
     int *hstate, *tbend;       // [S][143]
     uint32_t *v64_spec, *v64_end;   // [S][V64 chunks][32] chunk boundary metrics of the fast P1 Viterbi
     int *v64_endstate;         // [S]
-    int8_t *px_ring;           // [S][2 * IV_N] PX1 soft bits in arrival order (the last two interleaver spans)
+    int8_t *px_ring[2];        // [S][2 * IV_N] PX1 / PX2 (MP11) soft bits in arrival order (the last two interleaver spans)
     const uint32_t *iv_delay;  // [IV_N] interleaver IV: output m comes from the input iv_delay[m] positions earlier
-    int8_t *p3_vin;            // [S][8][13824] deinterleaved + depunctured P3 soft bits
-    uint2 *p3_dec;             // [S][8][P3_DEC_STRIDE] survivor decisions
-    uint32_t *p3_spec, *p3_end;     // [S][8][P3 chunks][32] fast Viterbi chunk boundary metrics
-    int *p3_endstate;          // [S][8]
-    uint2 *p3_fspec, *p3_fend; // [S][8][5][16] fallback Viterbi
-    int *p3_fhstate, *p3_ftbend;    // [S][8][5]
-    uint32_t *p3_bits;         // [S][8][144] decoded (still scrambled) bits
-    int *p3_flags;             // [S][8][4] ready, slow, retry, -
-    int8_t *px2_ring;          // [S][2 * IV_N] PX2 soft bits (MP11)
     const uint32_t *iv_delay_s;     // [IV_NS] interleaver IV of MP2 (J=2, M=4)
-    PxBufs xb[2];              // extra groups (null until the host enables them)
+    PxBufs xb[PX_GROUPS];      // per decode group (px_group)
     uint8_t *log;              // [S][log_cap]
     const float *shape;        // [2160]
     const float2 *twid;        // [FFT_TW] twiddle tables of fft2048_block (fft.cuh)

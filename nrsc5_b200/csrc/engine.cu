@@ -251,113 +251,31 @@ __host__ __device__ inline V64Args p1_v64_args(const DevPtrs &dp, int ch)
 }
 
 // ===========================================================================
-// P3 decode (MP3/MP11): for every P3 frame the pass queued (decode_push_px1, reference src/decode.c:393-414) -
-//   k_p3_gather : interleaver IV as a gather through its delay table + depuncture 1,0,1,1,0,1 (decode.c:344-376)
-//   the same Viterbi kernels as P1 (4608-bit frames: fast path with 256-step chunks, exact fallback)
-//   k_p3_fin    : descramble (decode.c:279-294) and pack into the frame's reserved record
-// P3 frames feed nothing back into the receiver (frame.c:535-540 only acts on P1), so they can wait for
-// the end of the pass.
+// Extended-partition decode (MP2, MP3, MP11): for every frame of decode group G (px_group) the pass queued
+// (decode_push_px1 / _px2, reference src/decode.c:393-437) -
+//   k_px_gather<G> : interleaver IV as a gather through its delay table + depuncture 1,0,1,1,0,1 (decode.c:344-376)
+//   the same Viterbi kernels as P1 (fast path with 256-step chunks, exact fallback)
+//   k_px_fin<G>    : descramble (decode.c:279-294) and pack into the frame's reserved record
+// These frames feed nothing back into the receiver (frame.c:535-540 only acts on P1), so they can wait for the end
+// of the pass.  G is a template argument so that the interleaver span is a compile-time divisor.
 // ===========================================================================
-__global__ void __launch_bounds__(256) k_p3_gather(DevPtrs p, EngineDims d)
+template <int G>
+__global__ void __launch_bounds__(256) k_px_gather(DevPtrs p, EngineDims d)
 {
+    constexpr int len = px_group(G).len, span = 32 * len;
     const int s = blockIdx.y, slot = blockIdx.x, t = threadIdx.x;
     const StreamState &st = p.st[s];
-    int *fl = p.p3_flags + ((size_t)s * P3_SLOTS + slot) * 4;
-    const bool on = slot < st.p3_pending;
-    if (t == 0) { fl[0] = on; fl[1] = 0; fl[2] = 0; }
-    if (!on) return;
-    const long long k0 = st.p3_k0[slot];
-    const int8_t *ring = p.px_ring + (size_t)s * PX_RING;
-    uint32_t *vout = reinterpret_cast<uint32_t *>(p.p3_vin + ((size_t)s * P3_SLOTS + slot) * P3_VIT);
-    // 12 outputs = 8 transmitted soft bits: positions 0 2 3 5 | 6 8 9 11 of each dozen, zeros in between
-    for (int g = t; g < P3_VIT / 12; g += 256) {
-        int8_t v[8];
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const long long k = k0 + 8 * g + i;
-            const long long j = k - (long long)__ldg(&p.iv_delay[k % IV_N]);
-            v[i] = ring[j % PX_RING];
-        }
-        auto b = [&](int i) { return (uint32_t)(uint8_t)v[i]; };
-        vout[3 * g + 0] = b(0) | (b(1) << 16) | (b(2) << 24);
-        vout[3 * g + 1] = (b(3) << 8) | (b(4) << 16);
-        vout[3 * g + 2] = b(5) | (b(6) << 8) | (b(7) << 24);
-    }
-}
-
-__global__ void __launch_bounds__(128) k_p3_fin(DevPtrs p, EngineDims d)
-{
-    const int s = blockIdx.y, slot = blockIdx.x, t = threadIdx.x;
-    const StreamState &st = p.st[s];
-    if (slot >= st.p3_pending) return;
-    const unsigned rec = st.p3_rec[slot];
-    if (rec == 0xffffffffu) return;
-    uint8_t *frame = p.log + (size_t)s * d.log_cap + rec + 8;          // past lc, nbits
-    const uint32_t *bw = p.p3_bits + ((size_t)s * P3_SLOTS + slot) * (P3_LEN / 32);
-    for (int w = t; w < P3_LEN / 32; w += 128) {
-        const uint32_t x = bw[w] ^ p.pnw[w];                            // the descrambler restarts with every frame
-        // MSB-first bytes
-        reinterpret_cast<uint32_t *>(frame)[w] = __brev(__byte_perm(x, 0, 0x0123));
-    }
-}
-
-__host__ __device__ inline V64Args p3_v64_args(const DevPtrs &dp)
-{
-    V64Args a;
-    a.vin = dp.p3_vin;
-    a.dec = dp.p3_dec;
-    a.vspec = dp.p3_spec;
-    a.vend = dp.p3_end;
-    a.endstate = dp.p3_endstate;
-    a.bitsw = dp.p3_bits;
-    a.ready = dp.p3_flags;
-    a.retry = dp.p3_flags + 2;
-    a.stride = 4;
-    a.len = P3_LEN;
-    a.ch = 256;
-    a.nch = (P3_LEN + 64 + 255) / 256;
-    a.dec_stride = P3_DEC_STRIDE;
-    return a;
-}
-
-__host__ __device__ inline VitcArgs p3_vitc_args(const DevPtrs &dp)
-{
-    VitcArgs a;
-    a.vin = dp.p3_vin;
-    a.dec = dp.p3_dec;
-    a.vspec = dp.p3_fspec;
-    a.vend = dp.p3_fend;
-    a.hstate = dp.p3_fhstate;
-    a.tbend = dp.p3_ftbend;
-    a.bitsw = dp.p3_bits;
-    a.ready = dp.p3_flags + 2;         // the fallback only decodes what the fast path gave up on
-    a.slow = dp.p3_flags + 1;
-    a.ready_stride = 4;
-    a.len = P3_LEN;
-    a.nch = (P3_LEN + 64 + CH_LEN - 1) / CH_LEN;
-    a.dec_stride = P3_DEC_STRIDE;
-    return a;
-}
-
-// ---- the extra extended-partition groups: MP2's 2304-bit P3 frames (which = 0: PX1 ring, interleaver IV with J=2,
-// M=4, span 73728) and MP11's P4 frames (which = 1: PX2 ring, the MP3 interleaver).  Same steps as the P3 group
-// above; the host adds them to a pass only after a stream has asked for them (g_px_need), so the hybrid modes pay
-// nothing for them.
-__global__ void __launch_bounds__(256) k_px_gather(DevPtrs p, EngineDims d, int which)
-{
-    const int s = blockIdx.y, slot = blockIdx.x, t = threadIdx.x;
-    const StreamState &st = p.st[s];
-    const PxBufs &xb = p.xb[which];
+    const PxBufs &xb = p.xb[G];
     int *fl = xb.flags + ((size_t)s * P3_SLOTS + slot) * 4;
-    const bool on = slot < st.xq_pending[which];
+    const bool on = slot < st.xq_pending[G];
     if (t == 0) { fl[0] = on; fl[1] = 0; fl[2] = 0; }
     if (!on) return;
-    const long long k0 = st.xq_k0[which][slot];
-    const int len = which == 0 ? P3S_LEN : P3_LEN, span = which == 0 ? IV_NS : IV_N;
-    const uint32_t *delay = which == 0 ? p.iv_delay_s : p.iv_delay;
-    const int8_t *ring = (which == 0 ? p.px_ring : p.px2_ring) + (size_t)s * PX_RING;
+    const long long k0 = st.xq_k0[G][slot];
+    const uint32_t *delay = len == P3_LEN ? p.iv_delay : p.iv_delay_s;
+    const int8_t *ring = p.px_ring[px_group(G).ring] + (size_t)s * PX_RING;
     uint32_t *vout = reinterpret_cast<uint32_t *>(xb.vin + ((size_t)s * P3_SLOTS + slot) * (3 * len));
-    for (int g = t; g < 3 * len / 12; g += 256) {           // depuncture 1,0,1,1,0,1 as in k_p3_gather
+    // 12 outputs = 8 transmitted soft bits: positions 0 2 3 5 | 6 8 9 11 of each dozen, zeros in between
+    for (int g = t; g < 3 * len / 12; g += 256) {
         int8_t v[8];
 #pragma unroll
         for (int i = 0; i < 8; i++) {
@@ -372,26 +290,28 @@ __global__ void __launch_bounds__(256) k_px_gather(DevPtrs p, EngineDims d, int 
     }
 }
 
-__global__ void __launch_bounds__(128) k_px_fin(DevPtrs p, EngineDims d, int which)
+template <int G>
+__global__ void __launch_bounds__(128) k_px_fin(DevPtrs p, EngineDims d)
 {
+    constexpr int len = px_group(G).len;
     const int s = blockIdx.y, slot = blockIdx.x, t = threadIdx.x;
     const StreamState &st = p.st[s];
-    if (slot >= st.xq_pending[which]) return;
-    const unsigned rec = st.xq_rec[which][slot];
+    if (slot >= st.xq_pending[G]) return;
+    const unsigned rec = st.xq_rec[G][slot];
     if (rec == 0xffffffffu) return;
-    const int len = which == 0 ? P3S_LEN : P3_LEN;
     uint8_t *frame = p.log + (size_t)s * d.log_cap + rec + 8;          // past lc, nbits
-    const uint32_t *bw = p.xb[which].bits + ((size_t)s * P3_SLOTS + slot) * (len / 32);
+    const uint32_t *bw = p.xb[G].bits + ((size_t)s * P3_SLOTS + slot) * (len / 32);
     for (int w = t; w < len / 32; w += 128) {
         const uint32_t x = bw[w] ^ p.pnw[w];                            // the descrambler restarts with every frame
+        // MSB-first bytes
         reinterpret_cast<uint32_t *>(frame)[w] = __brev(__byte_perm(x, 0, 0x0123));
     }
 }
 
-__host__ __device__ inline V64Args px_v64_args(const DevPtrs &dp, int which)
+__host__ __device__ inline V64Args px_v64_args(const DevPtrs &dp, int g)
 {
-    const PxBufs &xb = dp.xb[which];
-    const int len = which == 0 ? P3S_LEN : P3_LEN;
+    const PxBufs &xb = dp.xb[g];
+    const int len = px_group(g).len;
     V64Args a;
     a.vin = xb.vin;
     a.dec = xb.dec;
@@ -409,10 +329,10 @@ __host__ __device__ inline V64Args px_v64_args(const DevPtrs &dp, int which)
     return a;
 }
 
-__host__ __device__ inline VitcArgs px_vitc_args(const DevPtrs &dp, int which)
+__host__ __device__ inline VitcArgs px_vitc_args(const DevPtrs &dp, int g)
 {
-    const PxBufs &xb = dp.xb[which];
-    const int len = which == 0 ? P3S_LEN : P3_LEN;
+    const PxBufs &xb = dp.xb[g];
+    const int len = px_group(g).len;
     VitcArgs a;
     a.vin = xb.vin;
     a.dec = xb.dec;
@@ -421,7 +341,7 @@ __host__ __device__ inline VitcArgs px_vitc_args(const DevPtrs &dp, int which)
     a.hstate = xb.fhstate;
     a.tbend = xb.ftbend;
     a.bitsw = xb.bits;
-    a.ready = xb.flags + 2;
+    a.ready = xb.flags + 2;            // the fallback only decodes what the fast path gave up on
     a.slow = xb.flags + 1;
     a.ready_stride = 4;
     a.len = len;
@@ -1002,22 +922,8 @@ extern "C" int nrsc5b_create(nrsc5b_engine_t **out, const nrsc5b_config_t *cfg)
         DA(v64_end, uint32_t, (size_t)S * nch * 32);
         DA(v64_endstate, int, (size_t)S);
     }
-    {
-        const size_t F = (size_t)S * P3_SLOTS;
-        DA(px_ring, int8_t, (size_t)S * PX_RING);
-        DA(px2_ring, int8_t, (size_t)S * PX_RING);
-        DA(p3_vin, int8_t, F * P3_VIT);
-        DA(p3_dec, uint2, F * P3_DEC_STRIDE);
-        DA(p3_spec, uint32_t, F * 19 * 32);
-        DA(p3_end, uint32_t, F * 19 * 32);
-        DA(p3_endstate, int, F);
-        DA(p3_fspec, uint2, F * 5 * 16);
-        DA(p3_fend, uint2, F * 5 * 16);
-        DA(p3_fhstate, int, F * 5);
-        DA(p3_ftbend, int, F * 5);
-        DA(p3_bits, uint32_t, F * (P3_LEN / 32));
-        DA(p3_flags, int, F * 4);
-    }
+    DA(px_ring[0], int8_t, (size_t)S * PX_RING);
+    DA(px_ring[1], int8_t, (size_t)S * PX_RING);
     DA(log, uint8_t, (size_t)S * e->dims.log_cap);
     if (cfg->mode == NRSC5B_MODE_AM) {
         rc = dev_alloc(e, &e->am_st, (size_t)S);
@@ -1627,6 +1533,19 @@ static void launch_v64(const V64Args &a, int nframes, cudaStream_t stream)
     k_v64_emit<<<dim3((nwin + V64_EMIT_WARPS - 1) / V64_EMIT_WARPS, nframes), V64_EMIT_WARPS * 32, V64_EMIT_SMEM, stream>>>(a);
 }
 
+// Extended-partition decode group G, once a stream has asked for it (enable_px_groups).
+template <int G>
+static void launch_px_group(nrsc5b_engine *e)
+{
+    if (!(e->dims.px_enabled & (1 << G))) return;
+    const int S = e->dims.nstreams;
+    k_px_gather<G><<<dim3(P3_SLOTS, S), 256, 0, e->stream>>>(e->dp, e->dims);
+    launch_v64(px_v64_args(e->dp, G), S * P3_SLOTS, e->stream);
+    launch_vitc(px_vitc_args(e->dp, G), S * P3_SLOTS, e->stream);
+    k_px_fin<G><<<dim3(P3_SLOTS, S), 128, 0, e->stream>>>(e->dp, e->dims);
+    e->stats.kernel_launches += 8;
+}
+
 static void launch_p1(nrsc5b_engine *e)
 {
     NvtxRange nvtx_("nrsc5b: P1/P3 decode groups");
@@ -1636,34 +1555,20 @@ static void launch_p1(nrsc5b_engine *e)
     launch_vitc(p1_vitc_args(e->dp), S, e->stream);               // ... exact fallback for the frames it flagged
     k_p1_fin<<<dim3(FIN_CTAS, S), P1_THREADS, 0, e->stream>>>(e->dp, e->dims);
     e->stats.kernel_launches += 8;
-    // P3 / P4 frames: every group only once a stream has asked for it (enable_px_groups).  MP3 / MP11's 4608-bit P3:
-    if (e->dims.px_enabled & PX_NEED_P3) {
-        k_p3_gather<<<dim3(P3_SLOTS, S), 256, 0, e->stream>>>(e->dp, e->dims);
-        launch_v64(p3_v64_args(e->dp), S * P3_SLOTS, e->stream);
-        launch_vitc(p3_vitc_args(e->dp), S * P3_SLOTS, e->stream);
-        k_p3_fin<<<dim3(P3_SLOTS, S), 128, 0, e->stream>>>(e->dp, e->dims);
-        e->stats.kernel_launches += 8;
-    }
-    // MP2's short P3 frames / MP11's P4 frames
-    for (int which = 0; which < 2; which++) {
-        if (!(e->dims.px_enabled & (1 << which))) continue;
-        k_px_gather<<<dim3(P3_SLOTS, S), 256, 0, e->stream>>>(e->dp, e->dims, which);
-        launch_v64(px_v64_args(e->dp, which), S * P3_SLOTS, e->stream);
-        launch_vitc(px_vitc_args(e->dp, which), S * P3_SLOTS, e->stream);
-        k_px_fin<<<dim3(P3_SLOTS, S), 128, 0, e->stream>>>(e->dp, e->dims, which);
-        e->stats.kernel_launches += 8;
-    }
+    static_assert(PX_GROUPS == 3, "one launch per decode group, in group order");
+    launch_px_group<0>(e);
+    launch_px_group<1>(e);
+    launch_px_group<2>(e);
 }
 
-// Allocates the buffers of the extra decode groups named in `need` (PX_NEED_* bits) and adds them to the passes.
+// Allocates the buffers of the decode groups named in `need` (bit g = group g) and adds them to the passes.
 static int enable_px_groups(nrsc5b_engine *e, unsigned need)
 {
     const size_t F = (size_t)e->dims.nstreams * P3_SLOTS;
-    e->dims.px_enabled |= (int)(need & PX_NEED_P3);          // (its buffers exist from the start)
-    for (int which = 0; which < 2; which++) {
-        if (!(need & (1u << which)) || (e->dims.px_enabled & (1 << which))) continue;
-        const int len = which == 0 ? P3S_LEN : P3_LEN;
-        PxBufs &xb = e->dp.xb[which];
+    for (int g = 0; g < PX_GROUPS; g++) {
+        if (!(need & (1u << g)) || (e->dims.px_enabled & (1 << g))) continue;
+        const int len = px_group(g).len;
+        PxBufs &xb = e->dp.xb[g];
         int rc = dev_alloc(e, &xb.vin, F * 3 * len);
         if (!rc) rc = dev_alloc(e, &xb.dec, F * P3_DEC_STRIDE);
         if (!rc) rc = dev_alloc(e, &xb.spec, F * 19 * 32);
@@ -1676,7 +1581,7 @@ static int enable_px_groups(nrsc5b_engine *e, unsigned need)
         if (!rc) rc = dev_alloc(e, &xb.bits, F * (len / 32));
         if (!rc) rc = dev_alloc(e, &xb.flags, F * 4);
         if (rc) return rc;
-        e->dims.px_enabled |= 1 << which;
+        e->dims.px_enabled |= 1 << g;
     }
     return NRSC5B_OK;
 }

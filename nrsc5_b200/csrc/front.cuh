@@ -268,8 +268,7 @@ __device__ int front_prep_begin(const DevPtrs &p, const EngineDims &d, int s, in
             // P3 / P4 frames (MP2, MP3, MP11) are decoded by kernel groups the host adds to the pass only when a
             // stream asks: wait at the block boundary until it has (nrsc5b_process looks at the flag).  Streams
             // in MP1 / MP5 / MP6 never pay for those launches.
-            const int cm = c_compat_mode[st.psmi & 63];
-            const int need = cm == 2 ? PX_NEED_SHORT : cm == 3 ? PX_NEED_P3 : cm == 11 ? (PX_NEED_P3 | PX_NEED_PX2) : 0;
+            const int need = px_need_of(c_compat_mode[st.psmi & 63]);
             if (need & ~d.px_enabled) {
                 atomicOr(&p.ctl->px_need, (unsigned)need);
                 act = 0;
@@ -478,8 +477,7 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
             // P3 / P4 frames (MP2, MP3, MP11) are decoded by kernel groups the host adds to the pass only when a
             // stream asks: wait at the block boundary until it has (nrsc5b_process looks at the flag).  Streams
             // in MP1 / MP5 / MP6 never pay for those launches.
-            const int cm = c_compat_mode[st.psmi & 63];
-            const int need = cm == 2 ? PX_NEED_SHORT : cm == 3 ? PX_NEED_P3 : cm == 11 ? (PX_NEED_P3 | PX_NEED_PX2) : 0;
+            const int need = px_need_of(c_compat_mode[st.psmi & 63]);
             if (need & ~d.px_enabled) {
                 atomicOr(&p.ctl->px_need, (unsigned)need);
                 act = 0;
@@ -979,10 +977,8 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                     set_state(p, d, s, ST_FINE);
                     l2_enqueue(st, d.l2, 0u, 0, 0);            // frame_reset (sync.c:405-409)
                     st.started_pm = 0;                   // decode_reset (decode.c:556-565)
-                    st.px_total = 0;
-                    st.px_started = 0;
-                    st.px2_total = 0;
-                    st.px2_started = 0;
+                    st.px_total[0] = st.px_total[1] = 0;
+                    st.px_started[0] = st.px_started[1] = 0;
                 }
             } else if (st.cfo_wait == 0) {
                 sm.do_search = 1;
@@ -1279,10 +1275,10 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                 *reinterpret_cast<uint32_t *>(ring + pos) = w;
             }
         };
-        if (has_px1 && (st.px_started || (bc & 1) == 0))         // decode_push_px1, decode.c:393-399
-            px_demap(p.px_ring + (size_t)s * PX_RING, st.px_total, cm == 2 ? 2 : 4, 10, false);
-        if (cm == 11 && (st.px2_started || (bc & 1) == 0))       // decode_push_px2, decode.c:416-422
-            px_demap(p.px2_ring + (size_t)s * PX_RING, st.px2_total, 4, 12, true);
+        if (has_px1 && (st.px_started[0] || (bc & 1) == 0))      // decode_push_px1, decode.c:393-399
+            px_demap(p.px_ring[0] + (size_t)s * PX_RING, st.px_total[0], cm == 2 ? 2 : 4, 10, false);
+        if (cm == 11 && (st.px_started[1] || (bc & 1) == 0))     // decode_push_px2, decode.c:416-422
+            px_demap(p.px_ring[1] + (size_t)s * PX_RING, st.px_total[1], 4, 12, true);
         __syncthreads();
         if (t == 0) {
             st.err_lb += e_sb[0];
@@ -1337,57 +1333,29 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                 st.p1_ready = 1;
             }
             // P3 / P4 bookkeeping (decode_push_px1 / _px2, decode.c:393-437): every second block closes a span of the
-            // interleaver (9216 soft bits; MP2: 4608); once a whole cycle (147456; MP2: 73728) has gone through, it
-            // yields a frame.  The records are reserved now: P3 before P4, like the reference's calls.
-            if (has_px1) {
-                const int blk_len = cm == 2 ? PX1_BLOCK / 2 : PX1_BLOCK;
-                if ((bc & 1) == 0) st.px_started = 1;
-                if (st.px_started) {
-                    st.px_total += blk_len;
-                    const long long k0 = st.px_total - 2 * blk_len;
-                    if ((bc & 1) && cm != 2 && k0 >= IV_N && st.p3_pending < P3_SLOTS) {
-                        uint8_t *fw = log_reserve(p, d, s, REC_FRAME, 8 + P3_LEN / 8);
-                        const int e3 = st.p3_pending;
-                        st.p3_k0[e3] = k0;
-                        st.p3_rec[e3] = fw ? (unsigned)(fw - (p.log + (size_t)s * d.log_cap)) : 0xffffffffu;
-                        if (fw) {
-                            reinterpret_cast<uint32_t *>(fw)[0] = 1;        // P3 logical channel
-                            reinterpret_cast<uint32_t *>(fw)[1] = P3_LEN;
-                        }
-                        l2_enqueue(st, d.l2, fw ? st.p3_rec[e3] + 8 : 0xffffffffu, 1, P3_LEN);
-                        st.p3_pending = e3 + 1;
+            // interleaver (2 * len soft bits); once a whole cycle (32 * len) has gone through, it yields a frame.  A
+            // mode feeds at most one group per ring, so each ring advances once.  The records are reserved now, in
+            // group order: P3 before P4, like the reference's calls.  Unrolled, so that each group's constants fold:
+            // thread 0 runs this while the CTA waits, and a rolled loop costs MP3 streams measurably more.
+#pragma unroll
+            for (int g = 0; g < PX_GROUPS; g++) {
+                const PxGroup x = px_group(g);
+                if (!(x.modes >> cm & 1)) continue;
+                if ((bc & 1) == 0) st.px_started[x.ring] = 1;
+                if (!st.px_started[x.ring]) continue;
+                st.px_total[x.ring] += x.len;
+                const long long k0 = st.px_total[x.ring] - 2 * x.len;
+                if ((bc & 1) && k0 >= 32 * x.len && st.xq_pending[g] < P3_SLOTS) {
+                    uint8_t *fw = log_reserve(p, d, s, REC_FRAME, 8 + x.len / 8);
+                    const int e = st.xq_pending[g];
+                    st.xq_k0[g][e] = k0;
+                    st.xq_rec[g][e] = fw ? (unsigned)(fw - (p.log + (size_t)s * d.log_cap)) : 0xffffffffu;
+                    if (fw) {
+                        reinterpret_cast<uint32_t *>(fw)[0] = x.lc;
+                        reinterpret_cast<uint32_t *>(fw)[1] = x.len;
                     }
-                    if ((bc & 1) && cm == 2 && k0 >= IV_NS && st.xq_pending[0] < P3_SLOTS) {
-                        uint8_t *fw = log_reserve(p, d, s, REC_FRAME, 8 + P3S_LEN / 8);
-                        const int e3 = st.xq_pending[0];
-                        st.xq_k0[0][e3] = k0;
-                        st.xq_rec[0][e3] = fw ? (unsigned)(fw - (p.log + (size_t)s * d.log_cap)) : 0xffffffffu;
-                        if (fw) {
-                            reinterpret_cast<uint32_t *>(fw)[0] = 1;        // P3 logical channel
-                            reinterpret_cast<uint32_t *>(fw)[1] = P3S_LEN;
-                        }
-                        l2_enqueue(st, d.l2, fw ? st.xq_rec[0][e3] + 8 : 0xffffffffu, 1, P3S_LEN);
-                        st.xq_pending[0] = e3 + 1;
-                    }
-                }
-            }
-            if (cm == 11) {
-                if ((bc & 1) == 0) st.px2_started = 1;
-                if (st.px2_started) {
-                    st.px2_total += PX1_BLOCK;
-                    const long long k0 = st.px2_total - 2 * PX1_BLOCK;
-                    if ((bc & 1) && k0 >= IV_N && st.xq_pending[1] < P3_SLOTS) {
-                        uint8_t *fw = log_reserve(p, d, s, REC_FRAME, 8 + P3_LEN / 8);
-                        const int e4 = st.xq_pending[1];
-                        st.xq_k0[1][e4] = k0;
-                        st.xq_rec[1][e4] = fw ? (unsigned)(fw - (p.log + (size_t)s * d.log_cap)) : 0xffffffffu;
-                        if (fw) {
-                            reinterpret_cast<uint32_t *>(fw)[0] = 2;        // P4 logical channel
-                            reinterpret_cast<uint32_t *>(fw)[1] = P3_LEN;
-                        }
-                        l2_enqueue(st, d.l2, fw ? st.xq_rec[1][e4] + 8 : 0xffffffffu, 2, P3_LEN);
-                        st.xq_pending[1] = e4 + 1;
-                    }
+                    l2_enqueue(st, d.l2, fw ? st.xq_rec[g][e] + 8 : 0xffffffffu, x.lc, x.len);
+                    st.xq_pending[g] = e + 1;
                 }
             }
             st.bc = (bc + 1) % 16;
@@ -1439,9 +1407,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
     const bool owner = !CL || rank == 0;
     if (max_blocks > 16) max_blocks = 16;             // the PIDS queue (and its interleaver matrix rows) hold 16 blocks
     if (owner && t == 0) {                            // decoded by the kernels that followed the previous pass
-        st.p3_pending = 0;
-        st.xq_pending[0] = 0;
-        st.xq_pending[1] = 0;
+        for (int g = 0; g < PX_GROUPS; g++) st.xq_pending[g] = 0;
     }
     __syncthreads();
     for (int nb = 0;; nb++) {
