@@ -87,6 +87,10 @@ enum {
     NRSC5B_REC_BER = 6,       /* f32 cber                                  */
     NRSC5B_REC_SOFT_PM = 8,   /* u32 bc, 23040 int8 (only when enabled)    */
     NRSC5B_REC_BLOCK = 9,     /* i32 state_in, i32 samperr, f32 angle, f32 ph_re, f32 ph_im, i32 cfo, i64 start */
+    NRSC5B_REC_PAD = 12,      /* no payload, stands for no call: readers skip it.  FM keeps one after the P1 frame of a
+                               * block that also ends a P3 / P4 frame; if the P1 frame's header check fails, it becomes
+                               * REC_LOST_SYNC, so that the sync loss comes before those frames, as in the reference
+                               * (frame_push in decode_push_pm reports it before decode_push_px1 / _px2 run) */
     NRSC5B_REC_L2 = 20,       /* what frame_process() made of one frame (nrsc5b_enable_l2): u32 frame_off (log offset of the
                                * frame's packed bits in this drain; nrsc5b_l2_frames: index of the frame), u32 lc, u32 nbits,
                                * u32 pci, u32 flags (1: the sync-loss predicate of frame.c:535-540 fired, 2: event staging

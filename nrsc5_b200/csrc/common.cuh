@@ -58,7 +58,7 @@ constexpr int ST_NONE = 0, ST_COARSE = 1, ST_FINE = 2;
 
 // record types (include/nrsc5_b200.h)
 constexpr uint32_t REC_FRAME = 1, REC_PIDS = 2, REC_SYNC = 3, REC_LOST_SYNC = 4, REC_MER = 5,
-                   REC_BER = 6, REC_SOFT_PM = 8, REC_BLOCK = 9;
+                   REC_BER = 6, REC_SOFT_PM = 8, REC_BLOCK = 9, REC_PAD = 12;
 
 // bin index inside the compact 534-bin spectrum kept per symbol
 __host__ __device__ inline int compact_of_bin(int b)   // b in fftshift-ed coordinates
@@ -101,6 +101,7 @@ struct StreamState {
     int p1_slow;               // this frame needs saturating Viterbi arithmetic
     int p1_retry;              // the register-resident fast path could not prove its result: use the exact fallback kernels
     unsigned p1_rec;           // log offset of the reserved BER payload (FRAME record follows)
+    unsigned p1_lost_rec;      // log offset of the REC_PAD slot kept for the frame's sync loss, 0xffffffff = none
     int p1_errs;               // channel bit errors counted so far
     int p1_done;               // k_p1_fin CTAs finished
     int pids_pending;          // PIDS frames (of blocks pids_bc[]) waiting to be decoded into the log slots pids_rec[];

@@ -202,7 +202,14 @@ __global__ void __launch_bounds__(P1_THREADS) k_p1_fin(DevPtrs p, EngineDims d)
         const int ok = has_audio ? rs8_fix_header_warp(gf, hdr, t) : 1;
         if (t == 0) {
             if (rec) *reinterpret_cast<float *>(rec) = (float)atomicAdd(&st.p1_errs, 0) / (float)P1_ENC;
-            if (!ok) set_state(p, d, s, ST_NONE);
+            if (!ok) {
+                if (st.state == ST_FINE && st.p1_lost_rec != 0xffffffffu) {     // the slot k_stream kept between this
+                    *reinterpret_cast<uint32_t *>(p.log + (size_t)s * d.log_cap + st.p1_lost_rec) = REC_LOST_SYNC;
+                    st.state = ST_NONE;                                          // frame and its block's P3 / P4 frames
+                } else {
+                    set_state(p, d, s, ST_NONE);
+                }
+            }
             if (st.p1_retry) st.p1_fallbacks++;
             st.p1_ready = 0;
             st.p1_slow = 0;

@@ -1318,6 +1318,7 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             // P1 bookkeeping (decode.c:383-390); the BER and FRAME records are reserved now so that they keep
             // their place in the stream's record order (decode.c:458-460)
             if (bc == 0) st.started_pm = 1;
+            unsigned lost_slot = 0xffffffffu;
             if (st.started_pm && bc == 15) {
                 // both or neither: a BER record whose frame did not fit is taken back (its payload would never be filled)
                 const unsigned len0 = st.log_len;
@@ -1328,7 +1329,13 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                 if (fw) {
                     reinterpret_cast<uint32_t *>(fw)[0] = 0;            // P1 logical channel
                     reinterpret_cast<uint32_t *>(fw)[1] = P1_LEN;
+                    // the sync loss the frame's header check may report (k_p1_fin) comes before this block's P3 / P4
+                    // frames: the reference's frame_push reports it inside decode_push_pm, which runs before
+                    // decode_push_px1 / _px2.  Keep a slot for it here; it is taken back below if no such frame follows.
+                    uint8_t *lw = log_reserve(p, d, s, REC_PAD, 0);
+                    if (lw) lost_slot = (unsigned)(lw - 8 - (p.log + (size_t)s * d.log_cap));
                 }
+                st.p1_lost_rec = lost_slot;
                 l2_enqueue(st, d.l2, st.p1_rec != 0xffffffffu ? st.p1_rec + 4 + 8 + 8 : 0xffffffffu, 0, P1_LEN);   // BER payload | FRAME header | lc, nbits | bits
                 st.p1_ready = 1;
             }
@@ -1357,6 +1364,10 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                     l2_enqueue(st, d.l2, fw ? st.xq_rec[g][e] + 8 : 0xffffffffu, x.lc, x.len);
                     st.xq_pending[g] = e + 1;
                 }
+            }
+            if (lost_slot != 0xffffffffu && st.log_len == lost_slot + 8) {      // no P3 / P4 frame after it (MP1 logs
+                st.log_len = lost_slot;                                          // never hold the slot)
+                st.p1_lost_rec = 0xffffffffu;
             }
             st.bc = (bc + 1) % 16;
         }

@@ -174,6 +174,8 @@ static void replay(input_t *st, const uint8_t *rec, size_t n)
             frame_reset(&st->frame);
             break;
         }
+        case NRSC5B_REC_PAD:                         /* an unused slot: no call */
+            break;
         case NRSC5B_REC_LOST_SYNC:                   /* already reported if frame.c asked for it */
             if (st->sync_state == SYNC_STATE_FINE)
                 nrsc5_report_lost_sync(st->radio);

@@ -16,6 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 
 REC_FRAME, REC_PIDS, REC_SYNC, REC_LOST_SYNC, REC_MER, REC_BER = 1, 2, 3, 4, 5, 6
 REC_SOFT_PM, REC_BLOCK = 8, 9
+REC_PAD = 12                                                  # an unused slot: no call, parse_records skips it
 REC_L2 = 20                                                   # L2 framing of one frame (include/nrsc5_b200.h)
 EV_SERVICE, EV_ALIGN, EV_AAS, EV_PACKET = 16, 17, 18, 19      # its events: the reference's L2 -> L3 calls
 L2F_LOST, L2F_EV_OVERFLOW = 1, 2
@@ -156,11 +157,15 @@ def with_l2_in_call_order(raw: bytes):
 
 
 def parse_records(raw: bytes, offsets: list = None):
-    """Decode the engine's record stream into (type, dict) tuples (offsets: gets each record's byte offset)."""
+    """Decode the engine's record stream into (type, dict) tuples (offsets: gets each record's byte offset).
+    REC_PAD records stand for no call and are left out."""
     out = []
     off, n = 0, len(raw)
     while off < n:
         ty, plen = struct.unpack_from("<II", raw, off)
+        if ty == REC_PAD:
+            off += 8 + ((plen + 3) & ~3)
+            continue
         if offsets is not None:
             offsets.append(off)
         pay = raw[off + 8: off + 8 + plen]

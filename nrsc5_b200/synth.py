@@ -383,17 +383,20 @@ def make_fm(psmi: int = 1, nframes: int = 2, seed: int = 1234, lead_in: int = 10
             noise_lsb: float = 0.0, noise_seed: int = 5, rms_lsb: float = 20.0,
             tail_blocks: int = 2, valid_header: bool = True, pci: int = PCI_AUDIO,
             start_bc: int = 0, pids_crc: bool = False, p1_frames=None, p3_frames=None) -> FmCapture:
-    """FM capture (PSMI 1, 2, 3, 5, 6 or 11) holding `nframes` complete L1 frames
+    """FM capture of service mode `psmi` holding `nframes` complete L1 frames
     followed by `tail_blocks` further blocks so the last frame flushes
     (the reference has no flush call, SURVEY §3.5).
 
     What the reference does with the service modes (src/sync.c:343-357,537-595): MP2 = one more partition per
     sideband carrying P3 frames of 2304 bits (PX1); MP3 = two more, P3 frames of 4608 bits; MP11 = four more,
     PX1 as in MP3 plus PX2 with P4 frames of 4608 bits; MP5 / MP6 = fourteen partitions per sideband tracked,
-    equalised and counted in the MER, only the twenty main ones decoded (filled with unrelated QPSK here)."""
-    assert psmi in (1, 2, 3, 5, 6, 11)
+    equalised and counted in the MER, only the twenty main ones decoded (filled with unrelated QPSK here).
+    Any of the 64 PSMI values: the capture is laid out by its compatibility mode (compat_mode: 1, 2, 3, 5, 6 or 11)
+    and the reference subcarriers carry the raw value, which is what the receiver reports in its SYNC."""
+    cm = compat_mode(psmi)
+    assert 0 <= psmi < 64 and cm in (1, 2, 3, 5, 6, 11)
     rng = np.random.default_rng(seed)
-    nref = {1: 11, 2: 12, 3: 13, 5: 15, 6: 15, 11: 15}[psmi]
+    nref = {1: 11, 2: 12, 3: 13, 5: 15, 6: 15, 11: 15}[cm]
     nblocks = nframes * BLOCKS_PER_FRAME + tail_blocks
     idx_i = interleaver_i_index()
     idx_ii = interleaver_ii_index()
@@ -429,21 +432,21 @@ def make_fm(psmi: int = 1, nframes: int = 2, seed: int = 1234, lead_in: int = 10
     # (sync.c:537-595) and the bits they carry, [block][symbol][group][carrier][re, im]
     first_even = start_bc % 2                         # PX blocks before the first even block are read by nobody
     ext = []                                          # (bases, bits)
-    if psmi == 3:
+    if cm == 3:
         px1, cap.p3_frames = _px_stream(np.random.default_rng(seed + 7919), nblocks, first_even, PX1_BLOCK, p3_frames)
         ext.append(((LB_START + 190 + 1, LB_START + 209 + 1, UB_END - 228 + 1, UB_END - 209 + 1),
                     px1.reshape(nblocks, BLKSZ, 4, 18, 2)))
-    elif psmi == 2:
+    elif cm == 2:
         px1, cap.p3_frames = _px_stream(np.random.default_rng(seed + 7919), nblocks, first_even, PX1_BLOCK // 2)
         ext.append(((LB_START + 190 + 1, UB_END - 209 + 1), px1.reshape(nblocks, BLKSZ, 2, 18, 2)))
-    elif psmi == 11:
+    elif cm == 11:
         px1, cap.p3_frames = _px_stream(np.random.default_rng(seed + 7919), nblocks, first_even, PX1_BLOCK, p3_frames)
         px2, cap.p4_frames = _px_stream(np.random.default_rng(seed + 7920), nblocks, first_even, PX1_BLOCK)
         ext.append(((LB_START + 190 + 1, LB_START + 209 + 1, UB_END - 228 + 1, UB_END - 209 + 1),
                     px1.reshape(nblocks, BLKSZ, 4, 18, 2)))
         ext.append(((LB_START + 228 + 1, LB_START + 247 + 1, UB_END - 266 + 1, UB_END - 247 + 1),
                     px2.reshape(nblocks, BLKSZ, 4, 18, 2)))
-    elif psmi in (5, 6):
+    elif cm in (5, 6):
         fill = np.random.default_rng(seed + 7921).integers(0, 2, (nblocks, BLKSZ, 8, 18, 2), dtype=np.uint8)
         ext.append((tuple(LB_START + 19 * q + 1 for q in range(10, 14)) + tuple(UB_END - 19 * (q + 1) + 1 for q in range(13, 9, -1)),
                     fill))
