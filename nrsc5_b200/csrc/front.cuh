@@ -95,6 +95,21 @@ struct PrepSmem {
     int red_idx[FRONT_THREADS];
     float2 red_v[FRONT_THREADS];
 };
+// coarse acquisition by one CTA (front_prep_single): the window in tiles of one symbol period, so that term j of every
+// offset's cyclic-prefix correlation needs tiles j and j+1 only - the band-passed window never leaves the SM
+constexpr int ACQ1_RUN = 3;                        // odd: conflict-free; 731 runs cover NSYM + 31 outputs
+constexpr int ACQ1_WORDS = (NSYM + 38 + 3 + 3) / 4 * 4;   // a tile's cu8 words from a 16-byte boundary (word phase <= 3)
+static_assert(ACQ1_RUN * FRONT_THREADS >= NSYM + 31 && ACQ1_RUN % 2 == 1, "a tile's runs");
+struct Acq1Smem {
+    uint32_t words[2][ACQ1_WORDS];                 // cu8 of tiles j and j+1 (asynchronous copies, double-buffered)
+    short2 ytile[NSYM + 32];                       // tile j's halfband outputs, preceded by the 31 the band-pass looks back on
+    float2 ring[2][NSYM];                          // band-passed tiles j-1 and j: what the correlation reads
+    float2 sums[NSYM];
+    float2 shape[NCP];                             // (shape[j], shape[j + NFFT]) for the pulse-shaped sliding sum
+    float red_mag[FRONT_THREADS];
+    int red_idx[FRONT_THREADS];
+    float2 red_v[FRONT_THREADS];
+};
 struct PidsSmem {
     int8_t vit[PIDS_LEN * 3];
     uint2 dec[PIDS_LEN + 64];
@@ -134,6 +149,7 @@ struct FrontSmem {
     union {
         DemodSmem demod;
         PrepSmem prep;
+        Acq1Smem acq1;
         SyncSmem sync;
         PidsSmem pidsq[16];
     } u;
@@ -214,26 +230,44 @@ __device__ void front_pids_flush(const DevPtrs &p, const EngineDims &d, int s, P
 // ---------------------------------------------------------------------------
 // prep (reference src/acquire.c:98-168, src/sync.c:769-777, src/firdecim_q15.c:95-109,154-158)
 // ---------------------------------------------------------------------------
-// The decimated input of one acquisition tile: ytile[k] = y[i0 - 31 + k], k < L + 31, from the tile's words in sm.words
+// The decimated input of one acquisition tile: ytile[k] = y[i0 - 31 + k], k < L + 31, from the tile's words
 // (word v holds input samples 2 (start + i0 - 38 + v) and the next).  The window's first tile starts with the previous
-// window's last 31 outputs (bp_hist).  cu8: halfband_run over runs of ACQ_RUN outputs per thread; the last run is moved
+// window's last 31 outputs (bp_hist).  cu8: halfband_run over runs of RUN outputs per thread; the last run is moved
 // back to end at the tile's end and overlaps its neighbour's, writing the same values.
 constexpr int ACQ_RUN = 5;                         // odd: conflict-free; 1024 runs cover ACQ_TILE + 31 outputs
 static_assert(ACQ_RUN * FRONT_THREADS >= ACQ_TILE + 31, "a tile's runs");
-__device__ __forceinline__ void acq_tile_input(const EngineDims &d, PrepSmem &sm, const StreamState &st, int i0, int L, int t)
+template <int RUN>
+__device__ __forceinline__ void acq_tile_input(const EngineDims &d, const uint32_t *words, short2 *ytile, const StreamState &st,
+                                               int i0, int L, int t)
 {
     const int kb = i0 == 0 ? 31 : 0;
-    if (t < kb) sm.ytile[t] = make_short2(st.bp_hist[t][0], st.bp_hist[t][1]);
+    if (t < kb) ytile[t] = make_short2(st.bp_hist[t][0], st.bp_hist[t][1]);
     const int n = L + 31 - kb;
     if (d.cs16) {                                  // already decimated: the sample itself
         for (int k = kb + t; k < L + 31; k += FRONT_THREADS) {
-            const uint32_t w = sm.words[k + 7];
-            sm.ytile[k] = make_short2((short)(w & 0xffff), (short)(w >> 16));
+            const uint32_t w = words[k + 7];
+            ytile[k] = make_short2((short)(w & 0xffff), (short)(w >> 16));
         }
-    } else if (ACQ_RUN * t < n) {
-        const int k = kb + min(ACQ_RUN * t, n - ACQ_RUN);
-        halfband_run<ACQ_RUN>(sm.words + k, sm.ytile + k);
+    } else if (RUN * t < n) {
+        const int k = kb + min(RUN * t, n - RUN);
+        halfband_run<RUN>(words + k, ytile + k);
     }
+}
+
+// 32-tap symmetric Q15 band-pass (acquire.c:120-127, firdecim_q15.c:95-109) of output j of a tile: yy[k] = y[j - 31 + k]
+__device__ __forceinline__ float2 acq_bandpass(const short2 *yy)
+{
+    short accr = 0, acci = 0;
+#pragma unroll 5
+    for (int k = 1; k < 16; k++) {
+        const short2 a = yy[k], b = yy[32 - k];
+        accr = (short)(accr + ((((int)a.x + (int)b.x) * c_bp_tap[k]) >> 15));
+        acci = (short)(acci + ((((int)a.y + (int)b.y) * c_bp_tap[k]) >> 15));
+    }
+    const short2 c = yy[16];
+    accr = (short)(accr + (((int)c.x * c_bp_tap[16]) >> 15));
+    acci = (short)(acci + (((int)c.y * c_bp_tap[16]) >> 15));
+    return make_float2(__fdiv_rn((float)accr, 32767.0f), __fdiv_rn((float)acci, -32767.0f));
 }
 
 // NCO of a block in closed form, with the pulse shape folded in (acquire.c:243-252): nco[j] = shape[j] * exp(j*theta*j)
@@ -305,22 +339,9 @@ __device__ void front_acq_tiles(const DevPtrs &p, const EngineDims &d, int s, Pr
             sm.words[v] = a >= 0 ? __ldcg(iqw + a) : (d.cs16 ? 0u : 0x7f7f7f7fu);
         }
         __syncthreads();
-        acq_tile_input(d, sm, st, i0, L, t);
+        acq_tile_input<ACQ_RUN>(d, sm.words, sm.ytile, st, i0, L, t);
         __syncthreads();
-        for (int j = t; j < L; j += FRONT_THREADS) {
-            const short2 *yy = sm.ytile + j;                  // yy[k] = y[i - 31 + k]
-            short accr = 0, acci = 0;
-#pragma unroll 5
-            for (int k = 1; k < 16; k++) {
-                const short2 a = yy[k], b = yy[32 - k];
-                accr = (short)(accr + ((((int)a.x + (int)b.x) * c_bp_tap[k]) >> 15));
-                acci = (short)(acci + ((((int)a.y + (int)b.y) * c_bp_tap[k]) >> 15));
-            }
-            const short2 c = yy[16];
-            accr = (short)(accr + (((int)c.x * c_bp_tap[16]) >> 15));
-            acci = (short)(acci + (((int)c.y * c_bp_tap[16]) >> 15));
-            tb[i0 + j] = make_float2(__fdiv_rn((float)accr, 32767.0f), __fdiv_rn((float)acci, -32767.0f));
-        }
+        for (int j = t; j < L; j += FRONT_THREADS) tb[i0 + j] = acq_bandpass(sm.ytile + j);
         if (i0 + L == NACQ && t < 31) {                       // the window's last 31 outputs: the next window's history
             const short2 v = sm.ytile[L + t];
             st.bp_hist_next[t][0] = v.x;
@@ -460,7 +481,7 @@ __device__ void front_prep_finish(const DevPtrs &p, const EngineDims &d, int s, 
 // prep of a block by ONE CTA (k_stream<false>, a stream per CTA): everything front_prep_begin / front_acq_tiles /
 // front_acq_corr / front_prep_finish do, in one piece - kept as one function because the 128-stream kernel is at its
 // 64-register ceiling and the split version costs it spills
-__device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, PrepSmem &sm, float2 *nco, int t)
+__device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, Acq1Smem &sm, float2 *nco, int t)
 {
     StreamState &st = p.st[s];
     __shared__ int sh_active, sh_samperr;
@@ -493,53 +514,69 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
     const uint8_t *iq = p.iq + (size_t)s * d.in_stride;
     const int state_in = st.state;
     if (state_in != ST_FINE) {
-        float2 *tb = p.tbuf + (size_t)s * NACQ;
         const long long start = st.start;
-        const uint32_t *iqw = reinterpret_cast<const uint32_t *>(iq);
-        // the 71280-sample window in tiles: cu8 words -> shared memory (coalesced), halfband /2 (input.c:52-94),
-        // 32-tap symmetric Q15 band-pass (acquire.c:120-127, firdecim_q15.c:95-109) -> float window in `tb`
-        for (int i0 = 0; i0 < NACQ; i0 += ACQ_TILE) {
-            const int L = min(ACQ_TILE, NACQ - i0);
-            const long long w0 = start + i0 - 38;                 // word of halfband output i0-31's first input
-            for (int v = t; v < L + 38; v += FRONT_THREADS) {
-                const long long a = w0 + v;
-                // before the stream starts the decimator sees zeros = byte 127; through L2 only (asynchronous pushes)
-                sm.words[v] = a >= 0 ? __ldcg(iqw + a) : (d.cs16 ? 0u : 0x7f7f7f7fu);
-            }
-            __syncthreads();
-            acq_tile_input(d, sm, st, i0, L, t);
-            __syncthreads();
-            for (int j = t; j < L; j += FRONT_THREADS) {
-                const short2 *yy = sm.ytile + j;                  // yy[k] = y[i - 31 + k]
-                short accr = 0, acci = 0;
-#pragma unroll 5
-                for (int k = 1; k < 16; k++) {
-                    const short2 a = yy[k], b = yy[32 - k];
-                    accr = (short)(accr + ((((int)a.x + (int)b.x) * c_bp_tap[k]) >> 15));
-                    acci = (short)(acci + ((((int)a.y + (int)b.y) * c_bp_tap[k]) >> 15));
+        // the 71280-sample window in 33 tiles of one symbol period: cu8 words -> shared memory (asynchronous copies,
+        // tile j+1's in flight while tile j is filtered), halfband /2 (input.c:52-94), band-pass -> float tile in the
+        // ring.  Once tile j+1 is in the ring, term j of every offset's cyclic-prefix correlation (acquire.c:129-134)
+        // is added: y[j*NSYM + i] and y[j*NSYM + i + NFFT] lie in tiles j and j+1.  The thread of offset i adds its
+        // terms in j order, so every sum has the reference's order.
+        constexpr int NT = BLK + 1;
+        static_assert(NACQ == NT * NSYM, "the window is whole tiles");
+        const int woff = (int)((start - 38) & 3);                  // the same for every tile: NSYM is a multiple of 4
+        static_assert(NSYM % 4 == 0, "tiles start at the same word phase");
+        const int nvec = (woff + NSYM + 38 + 3) / 4;               // the 16-byte pieces that hold a needed word
+        auto fetch = [&](int T) {                                  // tile T's words, from the 16-byte boundary below
+            const long long w0 = start + (long long)T * NSYM - 38; // word of halfband output T*NSYM-31's first input
+            const long long w0a = w0 & ~3LL;
+            uint4 *dst = reinterpret_cast<uint4 *>(sm.words[T & 1]);
+            for (int v = t; v < nvec; v += FRONT_THREADS) {
+                const long long a = w0a + 4 * v;
+                if (a >= 0) {                                      // through L2 only: the input is advanced by asynchronous pushes
+#if defined(NB_EMU)
+                    dst[v] = *reinterpret_cast<const uint4 *>(iq + 4 * a);
+#else
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst + v)), "l"(iq + 4 * a) : "memory");
+#endif
+                } else {                                           // before the stream starts the decimator sees zeros = byte 127
+                    const uint32_t z = d.cs16 ? 0u : 0x7f7f7f7fu;
+                    dst[v] = make_uint4(z, z, z, z);
                 }
-                const short2 c = yy[16];
-                accr = (short)(accr + (((int)c.x * c_bp_tap[16]) >> 15));
-                acci = (short)(acci + (((int)c.y * c_bp_tap[16]) >> 15));
-                tb[i0 + j] = make_float2(__fdiv_rn((float)accr, 32767.0f), __fdiv_rn((float)acci, -32767.0f));
             }
-            if (i0 + L == NACQ && t < 31) {                       // keep the window's last 31 outputs as history
-                const short2 v = sm.ytile[L + t];
-                st.bp_hist[t][0] = v.x;
-                st.bp_hist[t][1] = v.y;
+#if !defined(NB_EMU)
+            asm volatile("cp.async.commit_group;" ::: "memory");
+#endif
+        };
+        for (int i = t; i < NSYM; i += FRONT_THREADS) sm.sums[i] = make_float2(0.f, 0.f);
+        if (t < NCP) sm.shape[t] = make_float2(__ldg(&p.shape[t]), __ldg(&p.shape[t + NFFT]));
+        fetch(0);
+#pragma unroll 1
+        for (int T = 0; T <= NT; T++) {                            // pass NT only adds the last term
+            if (T + 1 < NT) fetch(T + 1);                          // (its buffer was last read before the previous barrier)
+#if !defined(NB_EMU)
+            if (T + 1 < NT) asm volatile("cp.async.wait_group 1;" ::: "memory");
+            else asm volatile("cp.async.wait_group 0;" ::: "memory");
+#endif
+            __syncthreads();
+            if (T < NT) acq_tile_input<ACQ1_RUN>(d, sm.words[T & 1] + woff, sm.ytile, st, T * NSYM, NSYM, t);
+            if (T >= 2) {                                          // term j = T-2: tiles j and j+1, both in the ring
+                const float2 *ya = sm.ring[T & 1], *yb = sm.ring[(T - 1) & 1];
+                for (int i = t; i < NSYM; i += FRONT_THREADS) {
+                    const float2 a = ya[i], b = i + NFFT < NSYM ? ya[i + NFFT] : yb[i + NFFT - NSYM];
+                    const float2 pr = cmulf(a, make_float2(b.x, -b.y));
+                    sm.sums[i].x += pr.x;
+                    sm.sums[i].y += pr.y;
+                }
             }
             __syncthreads();
-        }
-        // cyclic-prefix correlation per sample offset (acquire.c:129-134)
-        for (int i = t; i < NSYM; i += FRONT_THREADS) {
-            float2 acc = make_float2(0.f, 0.f);
-            for (int j = 0; j < BLK; j++) {
-                float2 a = tb[i + j * NSYM], b = tb[i + j * NSYM + NFFT];
-                float2 pr = cmulf(a, make_float2(b.x, -b.y));
-                acc.x += pr.x;
-                acc.y += pr.y;
+            if (T < NT) {
+                float2 *y = sm.ring[T & 1];
+                for (int j = t; j < NSYM; j += FRONT_THREADS) y[j] = acq_bandpass(sm.ytile + j);
+                if (T == NT - 1 && t < 31) {                       // keep the window's last 31 outputs as history
+                    const short2 v = sm.ytile[NSYM + t];
+                    st.bp_hist[t][0] = v.x;
+                    st.bp_hist[t][1] = v.y;
+                }
             }
-            sm.sums[i] = acc;
         }
         __syncthreads();
         // pulse-shaped sliding sum and arg-max (acquire.c:136-151)
@@ -552,9 +589,9 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
                 int q = i + j;
                 if (q >= NSYM) q -= NSYM;
                 const float2 sv = sm.sums[q];
-                const float a = __ldg(&p.shape[j]), b = __ldg(&p.shape[j + NFFT]);
-                v.x += (sv.x * a) * b;
-                v.y += (sv.y * a) * b;
+                const float2 ab = sm.shape[j];
+                v.x += (sv.x * ab.x) * ab.y;
+                v.y += (sv.y * ab.x) * ab.y;
             }
             const float mag = v.x * v.x + v.y * v.y;
             if (mag > best) { best = mag; besti = i; bestv = v; }
@@ -1436,7 +1473,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         // first - which the stream's CTAs share
         int mode = 0;
         if (!CL) {
-            if (nb < max_blocks && !st.p1_ready) mode = front_prep_single(p, d, s, sm.u.prep, sm.nco, t) ? 1 : 0;
+            if (nb < max_blocks && !st.p1_ready) mode = front_prep_single(p, d, s, sm.u.acq1, sm.nco, t) ? 1 : 0;
             if (mode == 0) break;
         } else {
             if (owner) {
