@@ -308,6 +308,31 @@ int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes,
  * not be mixed with an asynchronous batch in flight (nrsc5b_submit .. nrsc5b_poll). */
 int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const uint8_t *cu8, size_t nbytes);
 
+/* cs16 wideband input: complex int16, I/Q interleaved (the nrsc5b_push_cs16 layout), at 23 814 000 S/s; 16 bits hold
+ * the 40-60 dB between a band's stations that 8 bits cannot.  The same taps W_k, phasor table P, N(T), carry rule and
+ * mixer index as cu8, no offset and unit gain (1 output LSB per input LSB):
+ *     acc = sum_{u<256} W_k[u] * x[32 n + u]   (exact, |acc| < 2^36);   v = sat16((acc + 2^18) >> 19);
+ *     y[k][n] = sat16((v * conj(P[(1600 m_k n) mod 11907]) + 2^14) >> 15)
+ * For x16 = 64 (x8 - 127) the output equals the cu8 output on x8 bit for bit ((64 a + 2^18) >> 19 == (a + 2^12) >> 13,
+ * and on cu8 input |v| < 2^15).  On cs16 input near full scale |v| can reach about 2^16; sat16 clamps it there.
+ * The format is fixed at create: a cu8 entry point called on a cs16 handle, or a cs16 one on a cu8 handle, returns
+ * NRSC5B_EINVAL and changes nothing.  nrsc5b_chan_destroy / _reset / _tables / _outputs are shared: the outputs of a
+ * capture of nvalues int16 values are nrsc5b_chan_outputs(nvalues) (nvalues / 2 samples, as nbytes / 2 for cu8).
+ * nvalues must be even (whole complex samples).  A cs16 handle owns 32 MiB + 2 KiB of device scratch, whatever the
+ * capture size: a staging buffer of 2^22 + 256 samples and the two byte planes (x = 256 x_hi + x_lo) the tensor cores
+ * read, made from it or from the caller's capture by a split pass. */
+int nrsc5b_chan_create_cs16(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch);
+/* host capture of nvalues int16 values -> host out[nch][2 * outputs]; synchronous (tests) */
+int nrsc5b_chan_run_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, int16_t *out);
+/* device capture (16-byte aligned) -> device out[nch][out_stride] as nrsc5b_chan_run_device writes it; asynchronous
+ * on cuda_stream.  The capture is only read (split into the handle's planes 2^17 outputs at a time). */
+int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *d_cs16, size_t nvalues, void *d_out, size_t out_stride,
+                                void *cuda_stream);
+/* nrsc5b_chan_push / nrsc5b_chan_feed for cs16: the same rules, nvalues int16 values (any alignment, host or device) */
+int nrsc5b_chan_push_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, void *d_out, size_t out_stride,
+                          void *cuda_stream, long long *nout);
+int nrsc5b_chan_feed_cs16(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const int16_t *cs16, size_t nvalues);
+
 const char *nrsc5b_version(void);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-"""ctypes binding of the wideband channeliser (include/nrsc5_b200.h, csrc/channelizer.cu): one cu8 capture at
+"""ctypes binding of the wideband channeliser (include/nrsc5_b200.h, csrc/channelizer.cu): one cu8 or cs16 capture at
 23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take.
 No CPU fallback: constructing a Channelizer without a CUDA device raises."""
 from __future__ import annotations
@@ -29,13 +29,18 @@ def _lib():
         L.nrsc5b_chan_reset.argtypes = [vp]
         L.nrsc5b_chan_push.argtypes = [vp, vp, sz, vp, sz, vp, ctypes.POINTER(ctypes.c_longlong)]
         L.nrsc5b_chan_feed.argtypes = [vp, vp, vp, vp, sz]
+        L.nrsc5b_chan_create_cs16.argtypes = [ctypes.POINTER(vp), ci, vp, ci]
+        L.nrsc5b_chan_run_device_cs16.argtypes = [vp, vp, sz, vp, sz, vp]
+        L.nrsc5b_chan_run_cs16.argtypes = [vp, vp, sz, vp]
+        L.nrsc5b_chan_push_cs16.argtypes = [vp, vp, sz, vp, sz, vp, ctypes.POINTER(ctypes.c_longlong)]
+        L.nrsc5b_chan_feed_cs16.argtypes = [vp, vp, vp, vp, sz]
         L._chan_ready = True
     return L
 
 
 def stream_outputs(pushed: int, nbytes: int) -> int:
-    """Outputs per channel a push of nbytes emits after `pushed` complex samples (include/nrsc5_b200.h):
-    N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0."""
+    """Outputs per channel a push of nbytes (cu8; cs16: int16 values) emits after `pushed` complex samples
+    (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0."""
     def n(t):
         return (t - TAPS) // DECIM + 1 if t >= TAPS else 0
     return n(pushed + nbytes // 2) - n(pushed)
@@ -51,16 +56,23 @@ def make_tables(offsets_100khz):
 
 
 def outputs(nbytes: int) -> int:
+    """Outputs per channel of a capture of nbytes cu8 bytes (or as many int16 values of cs16)."""
     return int(_lib().nrsc5b_chan_outputs(nbytes & ~63))
 
 
 class Channelizer:
-    def __init__(self, offsets_100khz, device: int = 0):
+    """input_cs16=False: the capture is cu8 (uint8, lengths in bytes); True: cs16 (int16, lengths in int16 values,
+    the _cs16 entry points).  Either way two input units make one complex sample."""
+    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False):
         self._L = _lib()
         self.offsets = np.ascontiguousarray(offsets_100khz, dtype=np.int32)
         self.nch = int(self.offsets.size)
+        self.input_cs16 = bool(input_cs16)
+        self._dtype = np.int16 if self.input_cs16 else np.uint8
+        self._sfx = "_cs16" if self.input_cs16 else ""
         self._h = ctypes.c_void_p()
-        _check(self._L.nrsc5b_chan_create(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), "nrsc5b_chan_create")
+        name = "nrsc5b_chan_create" + self._sfx
+        _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), name)
         self.device = device
         self.pushed = 0                 # T: complex samples pushed since create / reset (mirrors the handle's count)
 
@@ -87,18 +99,24 @@ class Channelizer:
         _check(self._L.nrsc5b_chan_tables(self._h, taps.ctypes.data, ph.ctypes.data), "nrsc5b_chan_tables")
         return taps, ph
 
+    def _call(self, name, *args):
+        name = name + self._sfx
+        return _check(getattr(self._L, name)(*args), name)
+
     def run(self, cu8: np.ndarray) -> np.ndarray:
-        """Host capture (uint8, I/Q interleaved) -> int16 array [nch][2 * outputs] (I, Q interleaved)."""
-        a = np.ascontiguousarray(cu8, dtype=np.uint8)
+        """Host capture (uint8, or int16 with input_cs16; I/Q interleaved) -> int16 array [nch][2 * outputs] (I, Q
+        interleaved)."""
+        a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
         n = outputs(a.size)
         out = np.empty((self.nch, 2 * max(n, 0)), dtype=np.int16)
         if n > 0:
-            _check(self._L.nrsc5b_chan_run(self._h, a.ctypes.data, a.size, out.ctypes.data), "nrsc5b_chan_run")
+            self._call("nrsc5b_chan_run", self._h, a.ctypes.data, a.size, out.ctypes.data)
         return out
 
     def run_device(self, d_cu8: int, nbytes: int, d_out: int, out_stride: int, stream: int = 0):
-        _check(self._L.nrsc5b_chan_run_device(self._h, ctypes.c_void_p(d_cu8), nbytes, ctypes.c_void_p(d_out), out_stride,
-                                             ctypes.c_void_p(stream)), "nrsc5b_chan_run_device")
+        """Device capture (nbytes bytes of cu8, or nbytes int16 values of cs16) -> d_out[nch][out_stride]."""
+        self._call("nrsc5b_chan_run_device", self._h, ctypes.c_void_p(d_cu8), nbytes, ctypes.c_void_p(d_out), out_stride,
+                   ctypes.c_void_p(stream))
 
     # ---- streaming: a capture pushed in pieces; the outputs concatenate to run() of the whole capture ----
     def reset(self):
@@ -106,19 +124,20 @@ class Channelizer:
         self.pushed = 0
 
     def push_device(self, ptr: int, nbytes: int, d_out: int, out_stride: int, stream: int = 0) -> int:
-        """The next nbytes of the capture at ptr (host or device memory) -> the outputs they complete, written to the
-        device buffer d_out[nch][out_stride] (int16 values); asynchronous on `stream`.  Returns the outputs per channel."""
+        """The next nbytes (cs16: int16 values) of the capture at ptr (host or device memory) -> the outputs they
+        complete, written to the device buffer d_out[nch][out_stride] (int16 values); asynchronous on `stream`.  Returns
+        the outputs per channel."""
         n = ctypes.c_longlong(0)
-        _check(self._L.nrsc5b_chan_push(self._h, ctypes.c_void_p(ptr), nbytes, ctypes.c_void_p(d_out), out_stride,
-                                        ctypes.c_void_p(stream), ctypes.byref(n)), "nrsc5b_chan_push")
+        self._call("nrsc5b_chan_push", self._h, ctypes.c_void_p(ptr), nbytes, ctypes.c_void_p(d_out), out_stride,
+                   ctypes.c_void_p(stream), ctypes.byref(n))
         self.pushed += nbytes // 2
         return int(n.value)
 
     def push(self, cu8: np.ndarray) -> np.ndarray:
-        """The next piece of the capture (uint8, I/Q interleaved, even length) -> int16 [nch][2 * n]: the outputs it
-        completes.  Synchronous."""
+        """The next piece of the capture (uint8, or int16 with input_cs16; I/Q interleaved, even length) -> int16
+        [nch][2 * n]: the outputs it completes.  Synchronous."""
         import torch
-        a = np.ascontiguousarray(cu8, dtype=np.uint8).reshape(-1)
+        a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
         n = stream_outputs(self.pushed, a.size)
         dev = torch.device("cuda", self.device)
         out = torch.empty((self.nch, 2 * max(n, 1)), dtype=torch.int16, device=dev)
@@ -130,19 +149,18 @@ class Channelizer:
 
     def feed(self, engine, data, streams=None):
         """The next piece of the capture -> channel k appended to cs16 stream streams[k] of `engine` (an Engine made
-        with input_cs16=True; streams None: stream k).  data: a uint8 numpy array or (pointer, nbytes) to host or device
-        memory.  Raises EngineError on NRSC5B_EFULL (nothing taken: process() and feed the same data again)."""
+        with input_cs16=True; streams None: stream k).  data: a uint8 (input_cs16: int16) numpy array or (pointer, nbytes
+        or int16 values) to host or device memory.  Raises EngineError on NRSC5B_EFULL (nothing taken: process() and feed the same data again)."""
         if isinstance(data, tuple):
             ptr, nbytes = int(data[0]), int(data[1])
             keep = None
         else:
-            keep = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+            keep = np.ascontiguousarray(data, dtype=self._dtype).reshape(-1)
             ptr, nbytes = (keep.ctypes.data if keep.size else 0), keep.size
         st = None
         if streams is not None:
             st = np.ascontiguousarray(streams, dtype=np.int32)
             if st.size != self.nch:
                 raise ValueError(f"streams: {st.size} entries for {self.nch} channels")
-        _check(self._L.nrsc5b_chan_feed(self._h, engine._h, None if st is None else st.ctypes.data, ctypes.c_void_p(ptr),
-                                        nbytes), "nrsc5b_chan_feed")
+        self._call("nrsc5b_chan_feed", self._h, engine._h, None if st is None else st.ctypes.data, ctypes.c_void_p(ptr), nbytes)
         self.pushed += nbytes // 2

@@ -29,6 +29,22 @@
 // turn, each issuing its tile's 16 wgmmas and then running the epilogue from its own registers (rounding, rotation,
 // saturation -> cs16 stores) while the other consumer's wgmmas run.  The 32 channels' taps (64 KB) stay in shared
 // memory for the CTA's lifetime; capture tiles go through a ring of four 32 KB stages.
+//
+// cs16 input (nrsc5b_chan_*_cs16): the same taps, phasor table, mixer index and output rounding, but no offset and
+// unit gain (1 output LSB per input LSB):
+//
+//     acc[k][n] = sum_{u < 256} W_k[u] * x[32 n + u]                              (exact: |acc| < 2^36)
+//     v         = sat16((acc + 2^18) >> 19)
+//     y[k][n]   = sat16((v * conj(P[(1600 m_k n) mod 11907]) + 2^14) >> 15)
+//
+// For x16 = 64 (x8 - 127) this is the cu8 definition bit for bit: (64 a + 2^18) >> 19 == (a + 2^12) >> 13, and the cu8
+// filter output stays below 2^28 (the table check below), so |v| < 2^15 there and sat16 does nothing.  On cs16 input
+// near full scale |v| reaches about 2^16 (sum |h| = 1.40); the saturation keeps the rotation's products in 32 bits.
+// The kernel splits every sample as x = 256 x_hi + x_lo (x_hi signed, x_lo unsigned bytes) into two planes laid out
+// like a cu8 capture (k_split_cs16, into handle-owned staging: TMA cannot address the bytes of an int16), reduces the
+// x_hi plane (wgmma s8 x s8) to A1 = sum W x_hi (|A1| < 2^28) in 32 registers, then the x_lo plane (wgmma u8 x s8)
+// to A2 = sum W x_lo (|A2| < 2^29) in the 64 accumulators, and combines acc = 256 A1 + A2 in exact 32-bit pieces
+// before the shared epilogue.  A tile's two planes take two consecutive stages of the ring.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -60,6 +76,11 @@ constexpr int HALF = PERIOD / 2 + 1;                              // phasor tabl
 constexpr uint32_t EPI_BYTES = ((HALF * 4 + 15) & ~15) + GROUP * 4 + 2 * GROUP * 4 + GROUP * 8;
 constexpr uint32_t SMEM_BYTES = W_BYTES + STAGES * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
 static_assert(SMEM_BYTES <= 227 * 1024, "more shared memory than an H100 block may have");
+// cs16: the byte planes of up to PLANE_SAMPLES samples, x_hi rows first, then x_lo rows (one TMA map over both)
+constexpr long long PLANE_SAMPLES = (1ll << 22) + 256;
+constexpr int PLANE_ROWS = (int)(2 * PLANE_SAMPLES / CHUNK);
+constexpr long long PIECE_OUT = 1ll << 17;                        // outputs per launch of the one-shot cs16 entry: 32 n + 224 <= PLANE_SAMPLES
+static_assert(DECIM * PIECE_OUT + TAPS - DECIM <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
 
 struct Params {
     int nch;                   // channels
@@ -141,14 +162,37 @@ __device__ __forceinline__ void wgmma_u8s8(uint32_t (&d)[64], uint64_t da, uint6
         : "l"(da), "l"(db), "r"(accumulate)
         : "memory");
 }
+// the same with a signed A (the x_hi plane of a cs16 capture)
+__device__ __forceinline__ void wgmma_s8s8(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate)
+        : "memory");
+}
 
 struct Barriers {
     uint64_t w_full, a_full[STAGES], a_empty[STAGES];
 };
 
+// CS16: map_x addresses the two byte planes of a cs16 capture, the x_lo plane PLANE_ROWS rows after the x_hi plane
+template <bool CS16>
 __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                                                            Params p)
 {
+    constexpr int PLANES = CS16 ? 2 : 1;                           // capture stages per tile
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t *smem_w = smem;                                        // [8 chunks][128 rows][64 B]
@@ -189,14 +233,15 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
             for (int c = 0; c < NCHUNK; c++)
                 tma_load_2d(smem_w + (size_t)c * TILE_N * CHUNK, &map_w, &bar.w_full, 0, (group * NCHUNK + c) * TILE_N);
             unsigned it = 0;
-            for (long long tile = slot; tile < p.tiles; tile += nslots, it++) {
-                const int s = it % STAGES;
-                if (it >= STAGES) mbar_wait(&bar.a_empty[s], (it / STAGES - 1) & 1);
-                mbar_expect_tx(&bar.a_full[s], A_STAGE_BYTES);
-                for (int c = 0; c < NCHUNK; c++)                 // K chunk c of output row n = capture-matrix row n + c
-                    tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, &map_x, &bar.a_full[s], 0,
-                                (int)(tile * TILE_M) + c);
-            }
+            for (long long tile = slot; tile < p.tiles; tile += nslots)
+                for (int pl = 0; pl < PLANES; pl++, it++) {      // cs16: the x_hi plane, then the x_lo plane
+                    const int s = it % STAGES;
+                    if (it >= STAGES) mbar_wait(&bar.a_empty[s], (it / STAGES - 1) & 1);
+                    mbar_expect_tx(&bar.a_full[s], A_STAGE_BYTES);
+                    for (int c = 0; c < NCHUNK; c++)             // K chunk c of output row n = capture-matrix row n + c
+                        tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, &map_x, &bar.a_full[s], 0,
+                                    (int)(tile * TILE_M) + c + pl * PLANE_ROWS);
+                }
         }
         return;
     }
@@ -207,11 +252,38 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
 #pragma unroll
     for (int i = 0; i < 8; i++) row[i] = p.out + s_dst[4 * i + q];
     mbar_wait(&bar.w_full, 0);
-    unsigned it = (unsigned)wg;
-    for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2) {
-        const int s = it % STAGES;
-        mbar_wait(&bar.a_full[s], (it / STAGES) & 1);
+    unsigned it = (unsigned)wg * PLANES;
+    for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2 * PLANES) {
         uint32_t d[64];                                            // (the first wgmma overwrites it: accumulate = 0)
+        int a1[32];                                                // cs16: A1 = sum W x_hi, [channel i][row h][re, im]
+        if constexpr (CS16) {
+            const int s = it % STAGES;
+            mbar_wait(&bar.a_full[s], (it / STAGES) & 1);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+            for (int c = 0; c < NCHUNK; c++)
+#pragma unroll
+                for (int k = 0; k < CHUNK / 32; k++) {
+                    const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
+                    const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)c * TILE_N * CHUNK, 32u * k);
+                    wgmma_s8s8(d, da, db, (c | k) ? 1u : 0u);
+                }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bar.a_empty[s]);
+            // |A1| <= 128 sum(|Wr| + |Wi|) < 2^28: the wrapped 32-bit 256 hi + lo is the value
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    a1[4 * i + 2 * h] = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h]);
+                    a1[4 * i + 2 * h + 1] = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h]);
+                }
+        }
+        const unsigned il = it + PLANES - 1;                       // the stage of the unsigned operand (cu8: the capture; cs16: x_lo)
+        const int s = il % STAGES;
+        mbar_wait(&bar.a_full[s], (il / STAGES) & 1);
         asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
         for (int c = 0; c < NCHUNK; c++)
@@ -243,9 +315,23 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
                 const bool up = qi >= (unsigned)HALF;
                 const short2 v2 = ph_half[up ? (unsigned)PERIOD - qi : qi];
                 const int phx = v2.x, phy = up ? -v2.y : v2.y;
-                const int ar = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h] - s_corr[2 * cl]);
-                const int ai = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h] - s_corr[2 * cl + 1]);
-                const int vr = (ar + (1 << (SHIFT1 - 1))) >> SHIFT1, vi = (ai + (1 << (SHIFT1 - 1))) >> SHIFT1;
+                int vr, vi;
+                if constexpr (CS16) {
+                    // acc = 256 A1 + A2 < 2^36; with A1 = 2^11 (A1 >> 11) + (A1 & 2047):
+                    // (acc + 2^18) >> 19 = (A1 >> 11) + ((256 (A1 & 2047) + A2 + 2^18) >> 19), all terms below 2^30
+                    const int a2r = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h]);           // |A2| < 2^29
+                    const int a2i = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h]);
+                    const int br = a1[4 * i + 2 * h], bi = a1[4 * i + 2 * h + 1];
+                    vr = (br >> 11) + ((((br & 2047) << 8) + a2r + (1 << 18)) >> 19);
+                    vi = (bi >> 11) + ((((bi & 2047) << 8) + a2i + (1 << 18)) >> 19);
+                    vr = vr > 32767 ? 32767 : (vr < -32768 ? -32768 : vr);                            // sat16: the rotation stays in 32 bits
+                    vi = vi > 32767 ? 32767 : (vi < -32768 ? -32768 : vi);
+                } else {
+                    const int ar = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h] - s_corr[2 * cl]);
+                    const int ai = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h] - s_corr[2 * cl + 1]);
+                    vr = (ar + (1 << (SHIFT1 - 1))) >> SHIFT1;
+                    vi = (ai + (1 << (SHIFT1 - 1))) >> SHIFT1;
+                }
                 int zr = vr * phx + vi * phy, zi = vi * phx - vr * phy;        // v * conj(P)
                 zr = (zr + (1 << 14)) >> 15;
                 zi = (zi + (1 << 14)) >> 15;
@@ -258,9 +344,29 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     }
 }
 
+// cs16 -> the two byte planes the kernel reads: x = 256 hi + lo, hi[v] = x[v] >> 8 (signed), lo[v] = x[v] & 255, v
+// counting int16 values (so each plane is laid out like a cu8 capture).  Four complex samples per thread; src 16-byte
+// aligned.
+__global__ void k_split_cs16(const int16_t *__restrict__ src, long long nvalues, uint8_t *__restrict__ hi, uint8_t *__restrict__ lo)
+{
+    const long long v0 = 8 * ((long long)blockIdx.x * blockDim.x + threadIdx.x);
+    if (v0 + 8 <= nvalues) {
+        const uint4 w = *reinterpret_cast<const uint4 *>(src + v0);
+        // little-endian: value 2j of a word is its bytes 0 (low), 1 (high); value 2j + 1 its bytes 2, 3
+        *reinterpret_cast<uint2 *>(hi + v0) = make_uint2(__byte_perm(w.x, w.y, 0x7531), __byte_perm(w.z, w.w, 0x7531));
+        *reinterpret_cast<uint2 *>(lo + v0) = make_uint2(__byte_perm(w.x, w.y, 0x6420), __byte_perm(w.z, w.w, 0x6420));
+    } else {
+        for (long long v = v0; v < nvalues; v++) {
+            hi[v] = (uint8_t)(src[v] >> 8);
+            lo[v] = (uint8_t)src[v];
+        }
+    }
+}
+
 // Streaming: after a launch over the staging buffer has used the outputs it could, the samples from 32 x (outputs) on -
-// at most 255 samples - move to the front of the buffer, where the next push's bytes are appended to them.  Source and
-// destination can overlap: one block reads everything before it writes.
+// at most 255 samples, 510 bytes of cu8 or 1020 of cs16 - move to the front of the buffer, where the next push's bytes
+// are appended to them.  Source and destination can overlap: one block (of nbytes / 2 threads or more) reads everything
+// before it writes.
 __global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
 {
     const int i = 2 * (int)threadIdx.x;
@@ -270,7 +376,8 @@ __global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
     if (i < nbytes) *reinterpret_cast<uint16_t *>(buf + i) = v;
 }
 
-constexpr size_t STAGE_CAP = (4u << 20) + 512;                    // staging: the carry (< 512 bytes) + 4 MiB of new capture
+constexpr size_t STAGE_CAP = (4u << 20) + 512;                    // cu8 staging: the carry (< 512 bytes) + 4 MiB of new capture
+constexpr size_t STAGE_CAP_CS16 = 4 * PLANE_SAMPLES;              // cs16 staging: as many samples as the planes hold (16 MiB + 1 KiB)
 constexpr int DST_RING = 8;                                       // destination tables in flight (nrsc5b_chan_feed)
 
 }  // namespace nbch
@@ -282,6 +389,7 @@ using namespace nbch;
 
 struct nrsc5b_channelizer {
     int device, nch, ngroups;
+    bool cs16;                            // the input format, fixed at create
     std::vector<int> offsets;             // m_k: channel offset from the capture centre in 100 kHz steps
     std::vector<int16_t> taps;            // [nch][TAPS][2] (Wr, Wi) of W_k[u]
     std::vector<short2> phasor;           // [PERIOD]
@@ -293,9 +401,10 @@ struct nrsc5b_channelizer {
     PFN_cuTensorMapEncodeTiled_v12000 encode;
     // streaming (nrsc5b_chan_push / nrsc5b_chan_feed)
     long long pushed;                     // T: complex samples pushed since create / reset
-    uint8_t *d_stage;                     // [STAGE_CAP]: carry (samples from 32 N(T) on) | the bytes being pushed
-    CUtensorMap map_stage;
-    cudaEvent_t stage_done;               // the last work that used d_stage (pushes may come on different CUDA streams)
+    uint8_t *d_stage;                     // [STAGE_CAP or STAGE_CAP_CS16]: carry (samples from 32 N(T) on) | the bytes being pushed
+    uint8_t *d_planes;                    // cs16: [2][PLANE_SAMPLES * 2] the x_hi and x_lo planes a launch reads
+    CUtensorMap map_stage;                // what a streamed launch reads: d_stage (cu8) or d_planes (cs16)
+    cudaEvent_t stage_done;               // the last work that used d_stage / d_planes (calls may come on different CUDA streams)
     long long *h_dst, *d_dst;             // [DST_RING][nch] page-locked / device: per-channel destinations of a feed
     cudaEvent_t dst_copied[DST_RING];
     unsigned dst_pos;
@@ -394,7 +503,7 @@ extern "C" int nrsc5b_chan_make_tables(const int *offsets_100khz, int nch, int16
     return NRSC5B_OK;
 }
 
-extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch)
+static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16)
 {
     if (!out || !offsets_100khz || nch <= 0 || nch > 4096) return NRSC5B_EINVAL;
     int ndev = 0;
@@ -407,9 +516,10 @@ extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const 
     c->device = device;
     c->nch = nch;
     c->ngroups = (nch + GROUP - 1) / GROUP;
+    c->cs16 = cs16;
     c->offsets.assign(offsets_100khz, offsets_100khz + nch);
     c->d_w = nullptr; c->d_rot = nullptr; c->d_corr = nullptr; c->d_phasor = nullptr;
-    c->pushed = 0; c->d_stage = nullptr; c->stage_done = nullptr;
+    c->pushed = 0; c->d_stage = nullptr; c->d_planes = nullptr; c->stage_done = nullptr;
     c->h_dst = nullptr; c->d_dst = nullptr; c->dst_pos = 0;
     for (int i = 0; i < DST_RING; i++) c->dst_copied[i] = nullptr;
     // driver entry point for the tensor-map encoder (no link-time dependency on libcuda)
@@ -438,24 +548,39 @@ extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const 
         ok = c->encode(&c->map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_w, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                        CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
-    // the streaming staging buffer as a [rows][64 B] capture matrix (rows past a launch's valid bytes only feed outputs
-    // the launch does not write)
-    ok = ok && cudaMalloc(&c->d_stage, STAGE_CAP) == cudaSuccess && cudaMemset(c->d_stage, 0, STAGE_CAP) == cudaSuccess &&
+    // the streaming staging buffer (cu8) or the cs16 byte planes as a [rows][64 B] capture matrix (rows past a launch's
+    // valid bytes only feed outputs the launch does not write)
+    const size_t stage_cap = cs16 ? STAGE_CAP_CS16 : STAGE_CAP, planes = cs16 ? 4 * PLANE_SAMPLES : 0;
+    ok = ok && cudaMalloc(&c->d_stage, stage_cap) == cudaSuccess && cudaMemset(c->d_stage, 0, stage_cap) == cudaSuccess &&
          cudaEventCreateWithFlags(&c->stage_done, cudaEventDisableTiming) == cudaSuccess;
+    if (ok && cs16) ok = cudaMalloc(&c->d_planes, planes) == cudaSuccess && cudaMemset(c->d_planes, 0, planes) == cudaSuccess;
     if (ok) {
-        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)(STAGE_CAP / CHUNK) };
+        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)((cs16 ? planes : STAGE_CAP) / CHUNK) };
         const cuuint64_t strides[1] = { CHUNK };
         const cuuint32_t box[2] = { CHUNK, TILE_M }, es[2] = { 1, 1 };
-        ok = c->encode(&c->map_stage, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_stage, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+        ok = c->encode(&c->map_stage, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, cs16 ? c->d_planes : c->d_stage, dims, strides, box, es,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
-    if (ok) ok = cudaFuncSetAttribute(k_channelize, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) == cudaSuccess;
+    if (ok)
+        ok = cudaFuncSetAttribute(cs16 ? k_channelize<true> : k_channelize<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)SMEM_BYTES) == cudaSuccess;
     if (!ok) {
         nrsc5b_chan_destroy(c);
         return NRSC5B_ECUDA;
     }
     *out = c;
     return NRSC5B_OK;
+}
+
+extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch)
+{
+    return create(out, device, offsets_100khz, nch, false);
+}
+
+extern "C" int nrsc5b_chan_create_cs16(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch)
+{
+    return create(out, device, offsets_100khz, nch, true);
 }
 
 extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
@@ -466,6 +591,7 @@ extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
     cudaFree(c->d_corr);
     cudaFree(c->d_phasor);
     cudaFree(c->d_stage);
+    cudaFree(c->d_planes);
     cudaFree(c->d_dst);
     if (c->h_dst) cudaFreeHost(c->h_dst);
     if (c->stage_done) cudaEventDestroy(c->stage_done);
@@ -490,8 +616,8 @@ static long long outputs_of(long long samples) { return samples < TAPS ? 0 : (sa
 /* How many output samples a capture of `nbytes` gives per channel: every output needs 256 input samples. */
 extern "C" long long nrsc5b_chan_outputs(size_t nbytes) { return outputs_of((long long)(nbytes / 2)); }
 
-// outputs n0 .. n0 + nout - 1 of the capture whose sample 32 n0 is row 0 of map_x: output n0 + j of channel k goes to
-// out + dst[k] + 2 j (dst null: k * out_stride)
+// outputs n0 .. n0 + nout - 1 of the capture whose sample 32 n0 is row 0 of map_x (cs16: of both planes in map_x):
+// output n0 + j of channel k goes to out + dst[k] + 2 j (dst null: k * out_stride)
 static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0, long long nout, int16_t *out, const long long *dst,
                   size_t out_stride, cudaStream_t stream)
 {
@@ -512,18 +638,33 @@ static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0,
     long long slots = sms / c->ngroups;
     if (slots < 1) slots = 1;
     if (slots > p.tiles) slots = p.tiles;
-    k_channelize<<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
+    if (c->cs16)
+        k_channelize<true><<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
+    else
+        k_channelize<false><<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
     return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
 }
 
-// The streaming core of nrsc5b_chan_push and nrsc5b_chan_feed: appends nbytes (even) of capture at `src` to the
-// handle's stream and writes the outputs they complete, N(T) .. N(T') - 1, output N(T) + j of channel k to
-// out + dst[k] + 2 j (dst: a device table; null: k * out_stride).  Pushes larger than the staging buffer go through it
-// in pieces.  Asynchronous on `stream`; the source is read by a copy on that stream.
-static int stream_in(nrsc5b_channelizer *c, const uint8_t *src, size_t nbytes, int16_t *out, const long long *dst, size_t out_stride,
+// cs16: the first nsamples (<= PLANE_SAMPLES) of the device capture at src (16-byte aligned) -> the handle's planes,
+// then outputs n0 .. n0 + nout - 1 of them as launch() writes them
+static int split_launch(nrsc5b_channelizer *c, const int16_t *src, long long nsamples, long long n0, long long nout, int16_t *out,
+                        const long long *dst, size_t out_stride, cudaStream_t stream)
+{
+    const long long nvalues = 2 * nsamples, threads = (nvalues + 7) / 8;
+    k_split_cs16<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(src, nvalues, c->d_planes, c->d_planes + 2 * PLANE_SAMPLES);
+    if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
+    return launch(c, c->map_stage, n0, nout, out, dst, out_stride, stream);
+}
+
+// The streaming core of nrsc5b_chan_push* and nrsc5b_chan_feed*: appends nsamples complex samples (cu8 or cs16, the
+// handle's format) at `src` to the handle's stream and writes the outputs they complete, N(T) .. N(T') - 1, output
+// N(T) + j of channel k to out + dst[k] + 2 j (dst: a device table; null: k * out_stride).  Pushes larger than the
+// staging buffer go through it in pieces.  Asynchronous on `stream`; the source is read by a copy on that stream.
+static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, int16_t *out, const long long *dst, size_t out_stride,
                      cudaStream_t stream)
 {
-    if (!nbytes) return NRSC5B_OK;
+    if (!nsamples) return NRSC5B_OK;
+    const size_t bps = c->cs16 ? 4 : 2, cap = (c->cs16 ? STAGE_CAP_CS16 : STAGE_CAP) / bps;   // bytes per sample, samples staged
     // device memory: a device-to-device copy; page-locked host memory: DMA straight from it; pageable host memory: the
     // driver stages it (the copy returns once it has read the caller's bytes)
     cudaPointerAttributes attr;
@@ -533,19 +674,23 @@ static int stream_in(nrsc5b_channelizer *c, const uint8_t *src, size_t nbytes, i
     const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;
     long long written = 0;
-    for (size_t done = 0; done < nbytes;) {
+    for (size_t done = 0; done < nsamples;) {
         const long long first = outputs_of(c->pushed);            // absolute index of staging row 0's output
-        const size_t carry = 2 * (size_t)(c->pushed - DECIM * first);
-        const size_t piece = (nbytes - done < STAGE_CAP - carry ? nbytes - done : STAGE_CAP - carry) & ~(size_t)1;
-        if (cudaMemcpyAsync(c->d_stage + carry, src + done, piece, kind, stream) != cudaSuccess) return NRSC5B_ECUDA;
-        const long long held = (long long)(carry + piece) / 2, nl = outputs_of(held);
+        const size_t carry = (size_t)(c->pushed - DECIM * first);
+        const size_t piece = nsamples - done < cap - carry ? nsamples - done : cap - carry;
+        if (cudaMemcpyAsync(c->d_stage + bps * carry, reinterpret_cast<const uint8_t *>(src) + bps * done, bps * piece, kind, stream) !=
+            cudaSuccess)
+            return NRSC5B_ECUDA;
+        const long long held = (long long)(carry + piece), nl = outputs_of(held);
         if (nl > 0) {
-            int rc = launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream);
+            int rc = c->cs16 ? split_launch(c, reinterpret_cast<const int16_t *>(c->d_stage), held, first, nl, out + 2 * written, dst,
+                                            out_stride, stream)
+                             : launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream);
             if (rc) return rc;
-            k_move_carry<<<1, 256, 0, stream>>>(c->d_stage, (size_t)CHUNK * nl, (int)(2 * (held - DECIM * nl)));
+            k_move_carry<<<1, (unsigned)(128 * bps), 0, stream>>>(c->d_stage, bps * DECIM * nl, (int)(bps * (held - DECIM * nl)));
             if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
         }
-        c->pushed += (long long)(piece / 2);
+        c->pushed += (long long)piece;
         written += nl;
         done += piece;
     }
@@ -559,24 +704,38 @@ extern "C" int nrsc5b_chan_reset(nrsc5b_channelizer_t *c)
     return NRSC5B_OK;
 }
 
-extern "C" int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, void *d_out, size_t out_stride,
-                                void *cuda_stream, long long *nout)
+// nsamples complex samples of the handle's format at src (checked by the caller)
+static int push(nrsc5b_channelizer *c, const void *src, size_t nsamples, void *d_out, size_t out_stride, void *cuda_stream, long long *nout)
 {
-    if (nout) *nout = 0;
-    if (!c || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
-    const long long n = outputs_of(c->pushed + (long long)(nbytes / 2)) - outputs_of(c->pushed);
+    const long long n = outputs_of(c->pushed + (long long)nsamples) - outputs_of(c->pushed);
     if (n > 0 && (!d_out || ((uintptr_t)d_out & 3) || (out_stride & 1) || (size_t)(2 * n) > out_stride)) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
-    const int rc = stream_in(c, cu8, nbytes, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride,
+    const int rc = stream_in(c, src, nsamples, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride,
                              reinterpret_cast<cudaStream_t>(cuda_stream));
     if (rc == NRSC5B_OK && nout) *nout = n;
     return rc;
 }
 
-extern "C" int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const uint8_t *cu8, size_t nbytes)
+extern "C" int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, void *d_out, size_t out_stride,
+                                void *cuda_stream, long long *nout)
 {
-    if (!c || !e || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
-    const long long n = outputs_of(c->pushed + (long long)(nbytes / 2)) - outputs_of(c->pushed);
+    if (nout) *nout = 0;
+    if (!c || c->cs16 || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
+    return push(c, cu8, nbytes / 2, d_out, out_stride, cuda_stream, nout);
+}
+
+extern "C" int nrsc5b_chan_push_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, void *d_out, size_t out_stride,
+                                     void *cuda_stream, long long *nout)
+{
+    if (nout) *nout = 0;
+    if (!c || !c->cs16 || (nvalues & 1) || (nvalues && !cs16)) return NRSC5B_EINVAL;
+    return push(c, cs16, nvalues / 2, d_out, out_stride, cuda_stream, nout);
+}
+
+// nsamples complex samples of the handle's format at src (checked by the caller)
+static int feed(nrsc5b_channelizer *c, nrsc5b_engine_t *e, const int *streams, const void *src, size_t nsamples)
+{
+    const long long n = outputs_of(c->pushed + (long long)nsamples) - outputs_of(c->pushed);
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const size_t nch = (size_t)c->nch;
     if (!c->h_dst) {
@@ -607,9 +766,21 @@ extern "C" int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, con
             return NRSC5B_ECUDA;
         c->dst_pos++;
     }
-    rc = stream_in(c, cu8, nbytes, t.base, d_dst, 0, t.stream);
+    rc = stream_in(c, src, nsamples, t.base, d_dst, 0, t.stream);
     if (rc) return rc;
     return nbfeed_commit(e, streams, c->nch, n);
+}
+
+extern "C" int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const uint8_t *cu8, size_t nbytes)
+{
+    if (!c || c->cs16 || !e || (nbytes & 1) || (nbytes && !cu8)) return NRSC5B_EINVAL;
+    return feed(c, e, streams, cu8, nbytes / 2);
+}
+
+extern "C" int nrsc5b_chan_feed_cs16(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const int16_t *cs16, size_t nvalues)
+{
+    if (!c || !c->cs16 || !e || (nvalues & 1) || (nvalues && !cs16)) return NRSC5B_EINVAL;
+    return feed(c, e, streams, cs16, nvalues / 2);
 }
 
 /* Device-resident capture (cu8, I/Q interleaved, 23 814 000 S/s; 64-byte aligned, nbytes of it valid) -> out[nch][out_stride]
@@ -617,7 +788,8 @@ extern "C" int nrsc5b_chan_feed(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, con
 extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8, size_t nbytes, void *d_out, size_t out_stride,
                                       void *cuda_stream)
 {
-    if (!c || !d_cu8 || !d_out || ((uintptr_t)d_cu8 & 63) || (nbytes & 63) || ((uintptr_t)d_out & 3) || (out_stride & 1)) return NRSC5B_EINVAL;
+    if (!c || c->cs16 || !d_cu8 || !d_out || ((uintptr_t)d_cu8 & 63) || (nbytes & 63) || ((uintptr_t)d_out & 3) || (out_stride & 1))
+        return NRSC5B_EINVAL;
     const long long nout = nrsc5b_chan_outputs(nbytes);
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
@@ -633,21 +805,40 @@ extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8
     return launch(c, map_x, 0, nout, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
-/* Host convenience (tests): host capture in, host cs16 out[nch][2 * outputs]. */
-extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, int16_t *out)
+/* Device-resident cs16 capture (16-byte aligned, nvalues even) -> out[nch][out_stride] as nrsc5b_chan_run_device writes it.
+ * Goes through the handle's planes PIECE_OUT outputs at a time; the caller's buffer is only read. */
+extern "C" int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *d_cs16, size_t nvalues, void *d_out, size_t out_stride,
+                                           void *cuda_stream)
 {
-    if (!c || !cu8 || !out) return NRSC5B_EINVAL;
-    nbytes &= ~(size_t)63;                                  // whole 64-byte rows (32 complex samples)
-    const long long nout = nrsc5b_chan_outputs(nbytes);
+    if (!c || !c->cs16 || !d_cs16 || !d_out || ((uintptr_t)d_cs16 & 15) || (nvalues & 1) || ((uintptr_t)d_out & 3) || (out_stride & 1))
+        return NRSC5B_EINVAL;
+    const long long nout = nrsc5b_chan_outputs(nvalues);      // nvalues / 2 samples, as nbytes / 2 for cu8
     if (nout <= 0) return NRSC5B_OK;
+    if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
+    if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    const int16_t *src = reinterpret_cast<const int16_t *>(d_cs16);
+    int16_t *out = reinterpret_cast<int16_t *>(d_out);
+    if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;   // the planes are shared with the stream
+    for (long long n0 = 0; n0 < nout; n0 += PIECE_OUT) {
+        const long long nl = nout - n0 < PIECE_OUT ? nout - n0 : PIECE_OUT;
+        const int rc = split_launch(c, src + 2 * DECIM * n0, DECIM * nl + TAPS - DECIM, n0, nl, out + 2 * n0, nullptr, out_stride, stream);
+        if (rc) return rc;
+    }
+    return cudaEventRecord(c->stage_done, stream) == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+}
+
+// host capture of `bytes` bytes -> device (padded to whole 64-byte rows) -> the format's device entry -> host out
+static int run_host(nrsc5b_channelizer *c, const void *in, size_t bytes, size_t count, long long nout, int16_t *out)
+{
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     uint8_t *d_in = nullptr;
     int16_t *d_out = nullptr;
-    const size_t padded = (nbytes + 63) & ~(size_t)63, stride = (size_t)(2 * nout);
+    const size_t padded = (bytes + 63) & ~(size_t)63, stride = (size_t)(2 * nout);
     int rc = NRSC5B_ECUDA;
     if (cudaMalloc(&d_in, padded + 64) == cudaSuccess && cudaMalloc(&d_out, (size_t)c->nch * stride * sizeof(int16_t)) == cudaSuccess &&
-        cudaMemset(d_in, 0, padded + 64) == cudaSuccess && cudaMemcpy(d_in, cu8, nbytes, cudaMemcpyHostToDevice) == cudaSuccess) {
-        rc = nrsc5b_chan_run_device(c, d_in, nbytes, d_out, stride, nullptr);
+        cudaMemset(d_in, 0, padded + 64) == cudaSuccess && cudaMemcpy(d_in, in, bytes, cudaMemcpyHostToDevice) == cudaSuccess) {
+        rc = c->cs16 ? nrsc5b_chan_run_device_cs16(c, d_in, count, d_out, stride, nullptr) : nrsc5b_chan_run_device(c, d_in, count, d_out, stride, nullptr);
         if (rc == NRSC5B_OK && cudaDeviceSynchronize() != cudaSuccess) {
             fprintf(stderr, "nrsc5_b200: channeliser kernel failed: %s\n", cudaGetErrorString(cudaGetLastError()));
             rc = NRSC5B_ECUDA;
@@ -658,4 +849,22 @@ extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size
     cudaFree(d_in);
     cudaFree(d_out);
     return rc;
+}
+
+/* Host convenience (tests): host capture in, host cs16 out[nch][2 * outputs]. */
+extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, int16_t *out)
+{
+    if (!c || c->cs16 || !cu8 || !out) return NRSC5B_EINVAL;
+    nbytes &= ~(size_t)63;                                  // whole 64-byte rows (32 complex samples)
+    const long long nout = nrsc5b_chan_outputs(nbytes);
+    if (nout <= 0) return NRSC5B_OK;
+    return run_host(c, cu8, nbytes, nbytes, nout, out);
+}
+
+extern "C" int nrsc5b_chan_run_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, int16_t *out)
+{
+    if (!c || !c->cs16 || !cs16 || !out || (nvalues & 1)) return NRSC5B_EINVAL;
+    const long long nout = nrsc5b_chan_outputs(nvalues);
+    if (nout <= 0) return NRSC5B_OK;
+    return run_host(c, cs16, 2 * nvalues, nvalues, nout, out);
 }
