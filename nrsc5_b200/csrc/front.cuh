@@ -120,10 +120,7 @@ constexpr int EQ_MAXPART = 12;                      // partitions per sideband t
                                                     // the two more of MP5/MP6/MP11 are equalised in place in global memory
 constexpr int EQ_ROWS = 2 * EQ_MAXPART * (PW - 1);  // data carriers of both sidebands
 struct SyncSmem {
-    // reference carriers after their Costas loop and the loop's phase, [symbol][reference slot]: the threads
-    // of a warp each walk one reference, symbol by symbol, so the slot index must be the contiguous one
-    float2 zref[BLK][ZS];
-    float phs[BLK][ZS];
+    float phs[BLK][ZS];                            // the Costas loop's phase, laid out like FrontSmem::zref
     float2 eph[2 * MAXREF][BLK];                   // exp(j*phs)
     float smag[2 * MAXREF];
     float cfq[2 * MAXREF];                         // Costas frequency of every reference after the block
@@ -139,13 +136,20 @@ struct SyncSmem {
     float fb_w[2][MAXREF], fb_xy[2][MAXREF + 1];   // feedback terms (phase differences, bin * frequency)
     float4 rowc[EQ_ROWS];                          // per carrier row: k*|upper ref|, (19-k)*|lower ref|, slots
     int ref_ok[2 * MAXREF], ref_bc[2 * MAXREF], ref_psmi[2 * MAXREF];
-    float mult[2];
-    float angle;
+    bool px_on[2];                                 // the block feeds PX1 / PX2, from interleaver position px_T
+    long long px_T[2];
+    uint8_t *soft_w;                               // REC_SOFT_PM payload
     int do_search;
 };
 struct FrontSmem {
     float2 tw[FFT_TW];                             // FFT twiddle tables (fft.cuh)
     float2 nco[NSYM];                              // window[j] * exp(j*theta*j) of the current block
+    // reference carriers [symbol][reference slot], stored by the demodulating teams beside the kept bins (outside the
+    // union: the sync phase reads them without a round trip through global memory), then rotated by the Costas loops.
+    // The threads of a warp each walk one reference, symbol by symbol, so the slot index is the contiguous one.
+    float2 zref[BLK][ZS];
+    signed char ref_slot[NBINS + 2];               // per kept bin: its reference slot, -1 = a data carrier
+    uint8_t ref_mask[128];                         // per demod thread: which of its kept-bin stores are reference carriers
     union {
         DemodSmem demod;
         PrepSmem prep;
@@ -682,7 +686,8 @@ __device__ __forceinline__ float2 sample_q15(short2 h)
 }
 
 __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sym, DemodSmem &sm, const float2 *nco,
-                            const float2 *tw, int half, int tl, long long start, int samperr, float theta, float2 phase0)
+                            const float2 *tw, float2 (*zref)[ZS], const signed char *ref_slot, const uint8_t *ref_mask,
+                            int half, int tl, long long start, int samperr, float theta, float2 phase0)
 {
     float2 *buf = sm.buf[half];
     uint8_t *in = reinterpret_cast<uint8_t *>(buf);
@@ -756,14 +761,23 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
     // kept bins (sync.c:785-789, fftshift defines.h:123-138): with q = tl + 128 h and natural bin k = q + 256 k3,
     //   k3 = 5 (q >= 222) -> compact q - 222,  k3 = 6 (q <= 232) -> q + 34      (lower sideband, bins 478..744)
     //   k3 = 1 (q >= 24)  -> compact q + 243,  k3 = 2 (q <= 34)  -> q + 499     (upper sideband, bins 1304..1570)
+    // The reference carriers also go to zref[sym]: bit 4 h + k of ref_mask[tl] marks the thread's k-th store of round h
+    // as one, ref_slot gives its slot.  (Tables rather than arithmetic on q: per-thread constants would be hoisted out
+    // of the symbol loop and spilled.)
     float2 *dst = p.bins + ((size_t)s * BLK + sym) * NBINS;
+    float2 *zr = zref[sym];
+    const unsigned mask = ref_mask[tl];
+    auto put = [&](int c, float2 v, int bit) {
+        dst[c] = v;
+        if (mask & (1u << bit)) zr[ref_slot[c]] = v;
+    };
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         const int q = tl + 128 * h;
-        if (q >= 222) dst[q - 222] = cmul(out[h][5], sp);
-        if (q <= 232) dst[q + 34] = cmul(out[h][6], sp);
-        if (q >= 24) dst[q + 243] = cmul(out[h][1], sp);
-        if (q <= 34) dst[q + 499] = cmul(out[h][2], sp);
+        if (q >= 222) put(q - 222, cmul(out[h][5], sp), 4 * h);
+        if (q <= 232) put(q + 34, cmul(out[h][6], sp), 4 * h + 1);
+        if (q >= 24) put(q + 243, cmul(out[h][1], sp), 4 * h + 2);
+        if (q <= 34) put(q + 499, cmul(out[h][2], sp), 4 * h + 3);
     }
 }
 
@@ -906,7 +920,7 @@ __device__ __forceinline__ int8_t soft_demap(float x, float mult)      // sync.c
 }
 
 template <bool CL>
-__device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSmem &sm, int t)
+__device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSmem &sm, float2 (*zref)[ZS], int t)
 {
     StreamState &st = p.st[s];
     float *cfreq = p.cfreq + (size_t)s * NFFT;
@@ -930,36 +944,51 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             sy0 = c1;
         }
     };
-    // data carriers of both sidebands -> shared memory as [carrier][symbol] (coalesced reads along the carriers)
+    // data carriers of both sidebands -> shared memory as [carrier][symbol] (coalesced reads along the carriers).
+    // Element idx = n * rows2 + r is walked incrementally, without a division per element: the staging warps share
+    // their schedulers with the Costas warp, whose chain is the phase's critical path.
     auto stage_eq = [&](int first, int stride) {
         const int rows = min(ppb, EQ_MAXPART) * (PW - 1), rows2 = 2 * rows;
+        const int dn = stride / rows2, dr = stride - dn * rows2;
+        int n = first / rows2, r = first - n * rows2;
 #pragma unroll 4
-        for (int idx = first; idx < rows2 * BLK; idx += stride) {
-            const int n = idx / rows2, r = idx - n * rows2;
+        for (; n < BLK;) {
             const int sb = r >= rows, rr = sb ? r - rows : r;
-            const int i = rr / (PW - 1), k = rr - i * (PW - 1) + 1;
-            const int ci = sb == 0 ? PW * i + k : (NBINS - 1 - PW) - PW * i + k;
+            const int i = rr / (PW - 1);
+            // lower: PW * i + k, upper: (NBINS - 1 - PW) - PW * i + k, with k = rr - (PW - 1) * i + 1
+            const int ci = sb == 0 ? rr + i + 1 : (NBINS - PW) + rr - (2 * PW - 1) * i;
             sm.eq[r][n] = ldbin(&bins[(size_t)n * NBINS + ci]);
+            r += dr;
+            n += dn;
+            if (r >= rows2) { r -= rows2; n++; }
         }
     };
     const bool pre_staged = st.state == ST_FINE && !(g_dbg & 1);   // partitions known: stage while warp 0 runs the Costas loops
-    // reference carriers -> shared memory, then one Costas loop per carrier (sync.c:359-363)
-    for (int i = t; i < ZS * BLK; i += FRONT_THREADS) {
-        const int slot = i & (ZS - 1), n = i / ZS;
-        const int ii = slot < MAXREF ? slot : slot - MAXREF;
-        if (slot < 2 * MAXREF && ii < nref) sm.zref[n][slot] = ldbin(&bins[(size_t)n * NBINS + compact_of_bin(ref_bin(slot))]);
+    // reference carriers: stored in zref by the demodulating teams; with a cluster per stream the helpers' symbols
+    // are only in global memory, so the owner gathers them all from there
+    if (CL) {
+        for (int i = t; i < ZS * BLK; i += FRONT_THREADS) {
+            const int slot = i & (ZS - 1), n = i / ZS;
+            const int ii = slot < MAXREF ? slot : slot - MAXREF;
+            if (slot < 2 * MAXREF && ii < nref) zref[n][slot] = ldbin(&bins[(size_t)n * NBINS + compact_of_bin(ref_bin(slot))]);
+        }
+        __syncthreads();
     }
-    __syncthreads();
     sylap(0);
+    // one Costas loop per reference carrier (sync.c:359-363), then its mean amplitude (calc_smag, sync.c:254-261:
+    // the FINE equaliser's, taken here from the same rotated row)
     if (t < 2 * MAXREF) {
         const int i = t < MAXREF ? t : t - MAXREF;
         if (i < nref) {
             const int b = ref_bin(t);
             float f = cfreq[b], ph = cphase[b];
-            costas_row(&sm.zref[0][t], &sm.phs[0][t], ZS, f, ph, 0, alpha, beta, !(g_dbg & 2));
+            costas_row(&zref[0][t], &sm.phs[0][t], ZS, f, ph, 0, alpha, beta, !(g_dbg & 2));
             cfreq[b] = f;
             cphase[b] = ph;
             sm.cfq[t] = f;
+            float sum = 0;
+            for (int n = 0; n < BLK; n++) sum += fabsf(zref[n][t].x);
+            sm.smag[t] = sum / BLK;
         }
     } else if (t >= 32 && pre_staged) {
         stage_eq(t - 32, FRONT_THREADS - 32);
@@ -972,7 +1001,7 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             const int i = t < MAXREF ? t : t - MAXREF;
             sm.ref_ok[t] = 0;
             if (i < nref) {
-                const float2 *z = &sm.zref[0][t];
+                const float2 *z = &zref[0][t];
                 const unsigned rsid = (unsigned)(30 - i) & 3;
                 bool ok = true;
                 unsigned raw = 0;
@@ -1036,7 +1065,7 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             for (int i = t; i < ZS * BLK; i += FRONT_THREADS) {
                 const int slot = i & (ZS - 1), n = i / ZS;
                 const int ii = slot < MAXREF ? slot : slot - MAXREF;
-                if (slot < 2 * MAXREF && ii < nref) bins[(size_t)n * NBINS + compact_of_bin(ref_bin(slot))] = sm.zref[n][slot];
+                if (slot < 2 * MAXREF && ii < nref) bins[(size_t)n * NBINS + compact_of_bin(ref_bin(slot))] = zref[n][slot];
             }
             for (int i = t; i < 76 * 22; i += FRONT_THREADS) sm.srch.offs[i / 22][i % 22] = -1;
             __syncthreads();
@@ -1124,66 +1153,16 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
     }
 
     if (st.state == ST_FINE) {
-        // reference amplitude per subcarrier (calc_smag, sync.c:254-261) and exp(j*phase) per (reference, symbol)
-        if (t < 2 * MAXREF) {
-            const int i = t < MAXREF ? t : t - MAXREF;
-            if (i < nref) {
-                float sum = 0;
-                for (int n = 0; n < BLK; n++) sum += fabsf(sm.zref[n][t].x);
-                sm.smag[t] = sum / BLK;
-            }
-        }
+        // exp(j*phase) per (reference, symbol), the equaliser's per-row constants, and the staging if it did not run
+        // beside the Costas loops
         for (int i = t; i < 2 * MAXREF * BLK; i += FRONT_THREADS) {
             const int slot = i >> 5, n = i & 31;
             const int ii = slot < MAXREF ? slot : slot - MAXREF;
             if (ii < nref) sm.eph[slot][n] = cexp_j(sm.phs[n][slot]);
         }
-        // timing / phase feedback (sync.c:426-463) on the last warp: the terms are computed in parallel, then
-        // summed by one lane in the reference's order (same values, same rounding as the sequential loop)
-        if (t >= FRONT_THREADS - 32) {
-            const int lane = t & 31;
-            if (lane < ppb) {
-                sm.fb_w[0][lane] = half_pi_wrap(sm.phs[0][lane], sm.phs[0][lane + 1]);
-                sm.fb_w[1][lane] = half_pi_wrap(sm.phs[0][MAXREF + lane + 1], sm.phs[0][MAXREF + lane]);
-            }
-            if (lane <= ppb) {
-                sm.fb_xy[0][lane] = (float)(LB0 + PW * lane - NFFT / 2) * sm.cfq[lane];
-                sm.fb_xy[1][lane] = (float)(UB1 - PW * lane - NFFT / 2) * sm.cfq[MAXREF + lane];
-            }
-            __syncwarp();
-            if (lane == 31) {
-                float samperr = 0, angle = 0, sum_xy = 0, sum_x2 = 0;
-                for (int i = 0; i < ppb; i++) {
-                    samperr += sm.fb_w[0][i];
-                    samperr += sm.fb_w[1][i];
-                }
-                // x / (2 pi) as a multiplication by the double reciprocal: the result is rounded to float anyway
-                const double inv_2pi = 1.0 / (2 * M_PI);
-                samperr = (float)((double)(samperr / (float)(ppb * 2) * (float)NFFT / (float)PW) * inv_2pi);
-                for (int i = 0; i <= ppb; i++) {
-                    float x;
-                    x = (float)(LB0 + PW * i - NFFT / 2);
-                    angle += sm.cfq[i]; sum_xy += sm.fb_xy[0][i]; sum_x2 += x * x;
-                    x = (float)(UB1 - PW * i - NFFT / 2);
-                    angle += sm.cfq[MAXREF + i]; sum_xy += sm.fb_xy[1][i]; sum_x2 += x * x;
-                }
-                samperr = (float)((double)samperr - (double)((sum_xy / sum_x2) * (float)NFFT) * inv_2pi * BLK);
-                st.samperr = (int)roundf(samperr);
-                angle /= (float)((ppb + 1) * 2);
-                st.angle = angle;
-                sm.angle = angle;
-            }
-        }
-        __syncthreads();
-        if (t < 2 * MAXREF) {
-            const int i = t < MAXREF ? t : t - MAXREF;
-            if (i < nref) cfreq[ref_bin(t)] = sm.cfq[t] - sm.angle;
-        }
         const int bc = st.bc;
         int8_t *pm = p.pm + ((size_t)s * 16 + bc) * PM_BLOCK;
         const int rows = min(ppb, EQ_MAXPART) * (PW - 1), rows2 = 2 * rows;
-        sylap(2);
-        if (!pre_staged) stage_eq(t, FRONT_THREADS);
         // per carrier row: the two interpolation weights and the reference slots on either side
         for (int r = t; r < rows2; r += FRONT_THREADS) {
             const int sb = r >= rows, rr = sb ? r - rows : r;
@@ -1193,6 +1172,17 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             else { slot_lo = MAXREF + i + 1; slot_hi = MAXREF + i; }
             sm.rowc[r] = make_float4((float)k * sm.smag[slot_hi], (float)(PW - k) * sm.smag[slot_lo],
                                      __int_as_float(slot_hi), __int_as_float(slot_lo));
+        }
+        sylap(2);
+        if (!pre_staged) stage_eq(t, FRONT_THREADS);
+        // the extended partitions' interleaver positions, read before thread 0 advances them below
+        const int cm = c_compat_mode[st.psmi & 63];
+        const bool has_px1 = cm == 2 || cm == 3 || cm == 11;
+        if (t == 0) {
+            sm.px_on[0] = has_px1 && (st.px_started[0] || (bc & 1) == 0);      // decode_push_px1, decode.c:393-399
+            sm.px_on[1] = cm == 11 && (st.px_started[1] || (bc & 1) == 0);     // decode_push_px2, decode.c:416-422
+            sm.px_T[0] = st.px_total[0];
+            sm.px_T[1] = st.px_total[1];
         }
         __syncthreads();
         sylap(3);
@@ -1238,7 +1228,8 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             if (r >= rows) e_ub += e;
             else e_lb += e;
         }
-        // modulation error per sideband: a fixed-shape tree (thread, warp shuffle, warp 0)
+        // modulation error per sideband: a fixed-shape tree (thread, warp shuffle, then warp 0's lane 0 over the warps'
+        // sums - which every warp repeats for itself and takes from its lane 0, instead of a barrier behind warp 0)
 #pragma unroll
         for (int o = 16; o; o >>= 1) {
             e_lb += __shfl_xor_sync(0xffffffffu, e_lb, o);
@@ -1246,78 +1237,116 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
         }
         if ((t & 31) == 0) { sm.wred[t >> 5][0] = e_lb; sm.wred[t >> 5][1] = e_ub; }
         __syncthreads();
-        float e_sb[2] = { 0.f, 0.f };
-        if (t < 32) {
-            float a = sm.wred[t][0], b = sm.wred[t][1];
+        float mult[2], e_sb[2];
+        {
+            const int lane = t & 31;
+            float a = sm.wred[lane][0], b = sm.wred[lane][1];
 #pragma unroll
             for (int o = 16; o; o >>= 1) {
                 a += __shfl_xor_sync(0xffffffffu, a, o);
                 b += __shfl_xor_sync(0xffffffffu, b, o);
             }
-            if (t == 0) {
-                e_sb[0] = a;
-                e_sb[1] = b;
-                const float mer_lb = 2.0f * BLK * (float)(ppb * 18) / a, mer_ub = 2.0f * BLK * (float)(ppb * 18) / b;
-                sm.mult[0] = fmaxf(fminf(mer_lb * 10, 127.0f), 1.0f);
-                sm.mult[1] = fmaxf(fminf(mer_ub * 10, 127.0f), 1.0f);
-            }
+            e_sb[0] = __shfl_sync(0xffffffffu, a, 0);
+            e_sb[1] = __shfl_sync(0xffffffffu, b, 0);
+            const float mer_lb = 2.0f * BLK * (float)(ppb * 18) / e_sb[0], mer_ub = 2.0f * BLK * (float)(ppb * 18) / e_sb[1];
+            mult[0] = fmaxf(fminf(mer_lb * 10, 127.0f), 1.0f);
+            mult[1] = fmaxf(fminf(mer_ub * 10, 127.0f), 1.0f);
         }
-        __syncthreads();
         sylap(4);
-        // soft demap (sync.c:509-536) of the 10 primary-main partitions of each sideband into the interleaver
-        // matrix, four soft bits (two carriers) per thread
-        for (int item = t; item < BLK * 20 * 9; item += FRONT_THREADS) {
-            const int n = item / 180, rem = item - n * 180;
-            const int part = rem / 9, c4 = rem - part * 9;             // part 0..19 in demap order
-            const int sb = part >= 10;
-            // lower sideband: partition index; upper: the reference walks them upwards, storage is downwards
-            const int r = (sb ? rows + (19 - part) * (PW - 1) : part * (PW - 1)) + 2 * c4;
-            const float mult = sm.mult[sb];
-            const float2 a = sm.eq[r][n], b = sm.eq[r + 1][n];
-            const unsigned w = (unsigned)(uint8_t)soft_demap(a.x, mult) | ((unsigned)(uint8_t)soft_demap(a.y, mult) << 8) |
-                               ((unsigned)(uint8_t)soft_demap(b.x, mult) << 16) | ((unsigned)(uint8_t)soft_demap(b.y, mult) << 24);
-            *reinterpret_cast<uint32_t *>(pm + n * 720 + part * 36 + 4 * c4) = w;
-        }
-        // Extended partitions (sync.c:537-595): MP2 = one more partition per sideband (PX1, 2304 soft bits per
-        // block), MP3 / MP11 = two more (PX1, 4608), MP11 = another two (PX2, 4608, both sidebands scaled with the
-        // LOWER sideband's factor, sync.c:591-592).  They go to the convolutional interleaver's store in arrival
-        // order.  The mode is looked up afresh here, so the block that reaches FINE sync demaps them although it
-        // did not equalise them (its partition count was fixed at entry): partitions the equaliser staged come
-        // from shared memory, the others from global memory (equalised in place above, or raw).
-        const int cm = c_compat_mode[st.psmi & 63];
-        const bool has_px1 = cm == 2 || cm == 3 || cm == 11;
-        const int eqparts = rows / (PW - 1);
-        auto px_demap = [&](int8_t *ring, long long T, int nq, int base, bool lower_scale_only) {
-            const int per_sym = nq * 36;
-            for (int item = t; item < BLK * nq * 9; item += FRONT_THREADS) {
-                const int n = item / (nq * 9), rem = item - n * (nq * 9);
-                const int q = rem / 9, c4 = rem - q * 9;
-                // nq == 4: lower base, lower base+1, upper base+1, upper base (counted from the band edge); nq == 2: lower, upper
-                const int sb = q >= nq / 2;
-                const int i = nq == 2 ? base : ((q == 0 || q == 3) ? base : base + 1);
-                float2 a, b;
-                if (i < eqparts) {
-                    const int r = (sb ? rows : 0) + i * (PW - 1) + 2 * c4;
-                    a = sm.eq[r][n];
-                    b = sm.eq[r + 1][n];
-                } else {
-                    const int ci = (sb == 0 ? PW * i : (NBINS - 1 - PW) - PW * i) + 1 + 2 * c4;
-                    a = ldbin(&bins[(size_t)n * NBINS + ci]);
-                    b = ldbin(&bins[(size_t)n * NBINS + ci + 1]);
-                }
-                const float mult = sm.mult[lower_scale_only ? 0 : sb];
-                const unsigned w = (unsigned)(uint8_t)soft_demap(a.x, mult) | ((unsigned)(uint8_t)soft_demap(a.y, mult) << 8) |
-                                   ((unsigned)(uint8_t)soft_demap(b.x, mult) << 16) | ((unsigned)(uint8_t)soft_demap(b.y, mult) << 24);
-                const long long pos = (T + n * per_sym + q * 36 + 4 * c4) % PX_RING;
-                *reinterpret_cast<uint32_t *>(ring + pos) = w;
+        // Warps 2..31 demap; meanwhile warp 0's thread 0 does the block's record bookkeeping and warp 1 the timing /
+        // phase feedback: neither touches what the demap reads, and both only feed the next block.
+        constexpr int DEMAP_T0 = 64;
+        if (t >= DEMAP_T0) {
+            const int td = t - DEMAP_T0;
+            constexpr int DSTRIDE = FRONT_THREADS - DEMAP_T0;
+            // soft demap (sync.c:509-536) of the 10 primary-main partitions of each sideband into the interleaver
+            // matrix, four soft bits (two carriers) per thread
+            for (int item = td; item < BLK * 20 * 9; item += DSTRIDE) {
+                const int n = item / 180, rem = item - n * 180;
+                const int part = rem / 9, c4 = rem - part * 9;             // part 0..19 in demap order
+                const int sb = part >= 10;
+                // lower sideband: partition index; upper: the reference walks them upwards, storage is downwards
+                const int r = (sb ? rows + (19 - part) * (PW - 1) : part * (PW - 1)) + 2 * c4;
+                const float ml = mult[sb];
+                const float2 a = sm.eq[r][n], b = sm.eq[r + 1][n];
+                const unsigned w = (unsigned)(uint8_t)soft_demap(a.x, ml) | ((unsigned)(uint8_t)soft_demap(a.y, ml) << 8) |
+                                   ((unsigned)(uint8_t)soft_demap(b.x, ml) << 16) | ((unsigned)(uint8_t)soft_demap(b.y, ml) << 24);
+                *reinterpret_cast<uint32_t *>(pm + n * 720 + part * 36 + 4 * c4) = w;
             }
-        };
-        if (has_px1 && (st.px_started[0] || (bc & 1) == 0))      // decode_push_px1, decode.c:393-399
-            px_demap(p.px_ring[0] + (size_t)s * PX_RING, st.px_total[0], cm == 2 ? 2 : 4, 10, false);
-        if (cm == 11 && (st.px_started[1] || (bc & 1) == 0))     // decode_push_px2, decode.c:416-422
-            px_demap(p.px_ring[1] + (size_t)s * PX_RING, st.px_total[1], 4, 12, true);
-        __syncthreads();
-        if (t == 0) {
+            // Extended partitions (sync.c:537-595): MP2 = one more partition per sideband (PX1, 2304 soft bits per
+            // block), MP3 / MP11 = two more (PX1, 4608), MP11 = another two (PX2, 4608, both sidebands scaled with the
+            // LOWER sideband's factor, sync.c:591-592).  They go to the convolutional interleaver's store in arrival
+            // order.  The mode is looked up afresh here, so the block that reaches FINE sync demaps them although it
+            // did not equalise them (its partition count was fixed at entry): partitions the equaliser staged come
+            // from shared memory, the others from global memory (equalised in place above, or raw).
+            const int eqparts = rows / (PW - 1);
+            auto px_demap = [&](int8_t *ring, long long T, int nq, int base, bool lower_scale_only) {
+                const int per_sym = nq * 36;
+                for (int item = td; item < BLK * nq * 9; item += DSTRIDE) {
+                    const int n = item / (nq * 9), rem = item - n * (nq * 9);
+                    const int q = rem / 9, c4 = rem - q * 9;
+                    // nq == 4: lower base, lower base+1, upper base+1, upper base (counted from the band edge); nq == 2: lower, upper
+                    const int sb = q >= nq / 2;
+                    const int i = nq == 2 ? base : ((q == 0 || q == 3) ? base : base + 1);
+                    float2 a, b;
+                    if (i < eqparts) {
+                        const int r = (sb ? rows : 0) + i * (PW - 1) + 2 * c4;
+                        a = sm.eq[r][n];
+                        b = sm.eq[r + 1][n];
+                    } else {
+                        const int ci = (sb == 0 ? PW * i : (NBINS - 1 - PW) - PW * i) + 1 + 2 * c4;
+                        a = ldbin(&bins[(size_t)n * NBINS + ci]);
+                        b = ldbin(&bins[(size_t)n * NBINS + ci + 1]);
+                    }
+                    const float ml = mult[lower_scale_only ? 0 : sb];
+                    const unsigned w = (unsigned)(uint8_t)soft_demap(a.x, ml) | ((unsigned)(uint8_t)soft_demap(a.y, ml) << 8) |
+                                       ((unsigned)(uint8_t)soft_demap(b.x, ml) << 16) | ((unsigned)(uint8_t)soft_demap(b.y, ml) << 24);
+                    const long long pos = (T + n * per_sym + q * 36 + 4 * c4) % PX_RING;
+                    *reinterpret_cast<uint32_t *>(ring + pos) = w;
+                }
+            };
+            if (sm.px_on[0]) px_demap(p.px_ring[0] + (size_t)s * PX_RING, sm.px_T[0], cm == 2 ? 2 : 4, 10, false);
+            if (sm.px_on[1]) px_demap(p.px_ring[1] + (size_t)s * PX_RING, sm.px_T[1], 4, 12, true);
+        } else if (t >= 32) {
+            // timing / phase feedback (sync.c:426-463): the terms are computed in parallel, then summed by one lane in
+            // the reference's order (same values, same rounding as the sequential loop)
+            const int lane = t & 31;
+            if (lane < ppb) {
+                sm.fb_w[0][lane] = half_pi_wrap(sm.phs[0][lane], sm.phs[0][lane + 1]);
+                sm.fb_w[1][lane] = half_pi_wrap(sm.phs[0][MAXREF + lane + 1], sm.phs[0][MAXREF + lane]);
+            }
+            if (lane <= ppb) {
+                sm.fb_xy[0][lane] = (float)(LB0 + PW * lane - NFFT / 2) * sm.cfq[lane];
+                sm.fb_xy[1][lane] = (float)(UB1 - PW * lane - NFFT / 2) * sm.cfq[MAXREF + lane];
+            }
+            __syncwarp();
+            float fb_angle = 0;
+            if (lane == 31) {
+                float samperr = 0, angle = 0, sum_xy = 0, sum_x2 = 0;
+                for (int i = 0; i < ppb; i++) {
+                    samperr += sm.fb_w[0][i];
+                    samperr += sm.fb_w[1][i];
+                }
+                // x / (2 pi) as a multiplication by the double reciprocal: the result is rounded to float anyway
+                const double inv_2pi = 1.0 / (2 * M_PI);
+                samperr = (float)((double)(samperr / (float)(ppb * 2) * (float)NFFT / (float)PW) * inv_2pi);
+                for (int i = 0; i <= ppb; i++) {
+                    float x;
+                    x = (float)(LB0 + PW * i - NFFT / 2);
+                    angle += sm.cfq[i]; sum_xy += sm.fb_xy[0][i]; sum_x2 += x * x;
+                    x = (float)(UB1 - PW * i - NFFT / 2);
+                    angle += sm.cfq[MAXREF + i]; sum_xy += sm.fb_xy[1][i]; sum_x2 += x * x;
+                }
+                samperr = (float)((double)samperr - (double)((sum_xy / sum_x2) * (float)NFFT) * inv_2pi * BLK);
+                st.samperr = (int)roundf(samperr);
+                angle /= (float)((ppb + 1) * 2);
+                st.angle = angle;
+                fb_angle = angle;
+            }
+            fb_angle = __shfl_sync(0xffffffffu, fb_angle, 31);
+            const int i = lane < MAXREF ? lane : lane - MAXREF;
+            if (lane < 2 * MAXREF && i < nref) cfreq[ref_bin(lane)] = sm.cfq[lane] - fb_angle;
+        } else if (t == 0) {
             st.err_lb += e_sb[0];
             st.err_ub += e_sb[1];
             if (++st.mer_cnt == 16) {
@@ -1331,22 +1360,12 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                 st.err_lb = 0;
                 st.err_ub = 0;
             }
-        }
-        if (d.emit_soft) {
-            __shared__ uint8_t *sh_w;
-            __syncthreads();
-            if (t == 0) {
-                sh_w = log_reserve(p, d, s, REC_SOFT_PM, 4 + PM_BLOCK);
-                if (sh_w) *reinterpret_cast<uint32_t *>(sh_w) = (uint32_t)bc;
+            if (d.emit_soft) {                  // filled below, once the demap is done
+                sm.soft_w = log_reserve(p, d, s, REC_SOFT_PM, 4 + PM_BLOCK);
+                if (sm.soft_w) *reinterpret_cast<uint32_t *>(sm.soft_w) = (uint32_t)bc;
             }
-            __syncthreads();
-            if (sh_w)
-                for (int o = t; o < PM_BLOCK; o += FRONT_THREADS) sh_w[4 + o] = (uint8_t)pm[o];
-            __syncthreads();
-        }
-        // PIDS (decode.c:463-471): the frames of a pass are decoded together when k_stream exits; the record
-        // slot is reserved here to keep the stream's record order
-        if (t == 0) {
+            // PIDS (decode.c:463-471): the frames of a pass are decoded together when k_stream exits; the record
+            // slot is reserved here to keep the stream's record order
             uint8_t *w = log_reserve(p, d, s, REC_PIDS, 11);             // 80 bits + CRC verdict
             const int e = st.pids_pending;
             st.pids_rec[e] = w ? (unsigned)(w - (p.log + (size_t)s * d.log_cap)) : 0xffffffffu;
@@ -1408,8 +1427,10 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
             }
             st.bc = (bc + 1) % 16;
         }
+        __syncthreads();
+        if (d.emit_soft && sm.soft_w)
+            for (int o = t; o < PM_BLOCK; o += FRONT_THREADS) sm.soft_w[4 + o] = (uint8_t)pm[o];
     }
-    __syncthreads();
     if (t == 0) {                                // window overlap carry (acquire.c:259-262)
         const int keep = NSYM + (NSYM / 2 - st.blk_samperr) + st.keep_extra;
         st.keep_extra = 0;
@@ -1450,6 +1471,18 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
     const int s = (int)blockIdx.x / C, rank = (int)blockIdx.x % C;
     StreamState &st = p.st[s];
     for (int i = t; i < FFT_TW; i += FRONT_THREADS) sm.tw[i] = __ldg(&p.twid[i]);
+    for (int c = t; c < NBINS; c += FRONT_THREADS)     // lower slot i: compact 19 i; upper slot MAXREF + i: 533 - 19 i
+        sm.ref_slot[c] = c < SIDE ? (c % PW == 0 ? c / PW : -1) : ((NBINS - 1 - c) % PW == 0 ? MAXREF + (NBINS - 1 - c) / PW : -1);
+    if (t < 128) {                                     // front_demod's stores of thread t: compact q-222, q+34, q+243, q+499
+        unsigned m = 0;
+        for (int h = 0; h < 2; h++) {
+            const int q = t + 128 * h;
+            const int c[4] = { q >= 222 ? q - 222 : -1, q <= 232 ? q + 34 : -1, q >= 24 ? q + 243 : -1, q <= 34 ? q + 499 : -1 };
+            for (int k = 0; k < 4; k++)
+                if (c[k] >= 0 && (c[k] < SIDE ? c[k] % PW == 0 : (NBINS - 1 - c[k]) % PW == 0)) m |= 1u << (4 * h + k);
+        }
+        sm.ref_mask[t] = (uint8_t)m;
+    }
     __syncthreads();
 
     const bool owner = !CL || rank == 0;
@@ -1512,7 +1545,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         }
 #pragma unroll 1
         for (int pass = 0; pass < BLK / (TEAMS * C); pass++)
-            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.tw, team, tl, start, samperr, theta, phase0);
+            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.tw, sm.zref, sm.ref_slot, sm.ref_mask, team, tl, start, samperr, theta, phase0);
         if (CL) {
             __threadfence();
             cluster_barrier();                        // every CTA's bins are in L2
@@ -1520,7 +1553,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         if (CL && !owner) continue;
         __syncthreads();
         lap(3);
-        front_sync<CL>(p, d, s, sm.u.sync, t);
+        front_sync<CL>(p, d, s, sm.u.sync, sm.zref, t);
         __syncthreads();
         lap(st.blk_state_in == ST_FINE ? 4 : 5);
     }
