@@ -245,31 +245,44 @@ __device__ __forceinline__ void l2_enqueue(StreamState &st, int l2_on, unsigned 
 //   y = x[2d-7] + sum_k ((x[2d-14+2k] + x[2d-2k]) * tap_k) >> 15,   x = (u8 - 127) * 64
 // i.e. per term (s * tap_k) >> 9 with s = u8 + u8 - 254, floored term by term as the reference does, plus 64 times the
 // centre sample.  |y| <= 256 * 25493 / 512 + 8192 < 32767: int accumulators are exact and never wrap.
-// The window slides one word per output, so each word is loaded and its bytes extracted once, not once per output
-// that uses it; the pair sums and products stay per output.  w[] and y[] may be shared or global memory.
+// The window slides one word per output, so each word is loaded once, not once per output that uses it.  The bytes
+// are never extracted: one byte permute puts the real and imaginary bytes of a tap pair side by side, and a
+// two-way dot product with the tap in both 16-bit halves of `a` forms (u8 + u8) * tap - 254 * tap in one instruction
+// per component (the bias is its addend); the centre term is a dot product with 64 as well.  Every product is the
+// exact integer of the form above.  w[] and y[] may be shared or global memory.
+//
+// dp2a: c + a.h0 * b.b0 + a.h1 * b.b1 (HI = false) or b.b2, b.b3 (HI = true), a's halves signed, b's bytes unsigned
+template <bool HI>
+__device__ __forceinline__ int dp2a_su(int a, uint32_t b, int c)
+{
+#if defined(NB_EMU)
+    const int s = HI ? 16 : 0;
+    return c + (int)(short)(a & 0xffff) * (int)((b >> s) & 0xffu) + (int)(short)(a >> 16) * (int)((b >> (s + 8)) & 0xffu);
+#else
+    int d;
+    if (HI) asm("dp2a.hi.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    else    asm("dp2a.lo.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    return d;
+#endif
+}
+
 template <int R>
 __device__ __forceinline__ void halfband_run(const uint32_t *w, short2 *y)
 {
     const int tap[4] = { -134, 1078, -4417, 19864 };
-    int lr[R + 7], li[R + 7];                     // low half of word q: the real and imaginary byte of sample 2q
-    int cr[R], ci[R];                             // high half of word r + 3: the centre sample of output r
+    uint32_t v[R + 7];
 #pragma unroll
-    for (int q = 0; q < R + 7; q++) {
-        const uint32_t v = w[q];
-        lr[q] = (int)(v & 0xffu);
-        li[q] = (int)((v >> 8) & 0xffu);
-        if (q >= 3 && q < R + 3) {
-            cr[q - 3] = (int)((v >> 16) & 0xffu);
-            ci[q - 3] = (int)(v >> 24);
-        }
-    }
+    for (int q = 0; q < R + 7; q++) v[q] = w[q];
 #pragma unroll
     for (int r = 0; r < R; r++) {
-        int ar = cr[r] * 64 - 127 * 64, ai = ci[r] * 64 - 127 * 64;
+        // 64 x[2r+7] - 127 * 64, from the high half of word r + 3
+        int ar = dp2a_su<true>(64, v[r + 3], -127 * 64), ai = dp2a_su<true>(64 << 16, v[r + 3], -127 * 64);
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            ar += ((lr[r + k] + lr[r + 7 - k]) * tap[k] - 254 * tap[k]) >> 9;
-            ai += ((li[r + k] + li[r + 7 - k]) * tap[k] - 254 * tap[k]) >> 9;
+            const uint32_t pr = __byte_perm(v[r + k], v[r + 7 - k], 0x5140);   // re(2(r+k)), re(2(r+7-k)), im, im
+            const int tt = (tap[k] & 0xffff) | (tap[k] << 16);
+            ar += dp2a_su<false>(tt, pr, -254 * tap[k]) >> 9;
+            ai += dp2a_su<true>(tt, pr, -254 * tap[k]) >> 9;
         }
         y[r] = make_short2((short)ar, (short)ai);
     }

@@ -115,6 +115,7 @@ struct PidsSmem {
     uint2 dec[PIDS_LEN + 64];
 };
 constexpr int ZS = 32;                              // row stride of the per-reference arrays (>= 2 * MAXREF)
+static_assert(2 * MAXREF <= 32, "a reference slot fits the 5 bits of FrontSmem::ref_plan");
 constexpr int EQ_LD = BLK + 1;                      // padded row of the equalisation buffer (bank-conflict free)
 constexpr int EQ_MAXPART = 12;                      // partitions per sideband the equaliser stages in shared memory (MP1..MP3);
                                                     // the two more of MP5/MP6/MP11 are equalised in place in global memory
@@ -148,8 +149,7 @@ struct FrontSmem {
     // union: the sync phase reads them without a round trip through global memory), then rotated by the Costas loops.
     // The threads of a warp each walk one reference, symbol by symbol, so the slot index is the contiguous one.
     float2 zref[BLK][ZS];
-    signed char ref_slot[NBINS + 2];               // per kept bin: its reference slot, -1 = a data carrier
-    uint8_t ref_mask[128];                         // per demod thread: which of its kept-bin stores are reference carriers
+    uint8_t ref_plan[128];                         // per demod thread: which of its kept-bin stores is a reference carrier, and its slot
     union {
         DemodSmem demod;
         PrepSmem prep;
@@ -686,7 +686,7 @@ __device__ __forceinline__ float2 sample_q15(short2 h)
 }
 
 __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sym, DemodSmem &sm, const float2 *nco,
-                            const float2 *tw, float2 (*zref)[ZS], const signed char *ref_slot, const uint8_t *ref_mask,
+                            const float2 *tw, float2 (*zref)[ZS], const uint8_t *ref_plan,
                             int half, int tl, long long start, int samperr, float theta, float2 phase0)
 {
     float2 *buf = sm.buf[half];
@@ -701,18 +701,24 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
     {
         // the symbol's cu8 bytes go to shared memory by asynchronous 16-byte copies (cp.async.cg: through L2 only - samples
         // may have landed after an earlier, partial read of the same line - and past the register file)
+        // Vector v = tl + 128 i of the thread: four of them, and a fifth below nvec (542 or 543) - unrolled, with the
+        // addresses at constant offsets.  Only the stream's first symbols (b0a < 0) test each vector for the history.
         const int nvec = (off + 4 * NSYM + 28 + 15) / 16;
-        uint4 *dst = reinterpret_cast<uint4 *>(in);
-        for (int v = tl; v < nvec; v += 128) {
-            const long long a = b0a + 16LL * v;
-            if (a >= 0) {
+        static_assert(4 * 128 < (4 * NSYM + 28 + 15) / 16 && (12 + 4 * NSYM + 28 + 15) / 16 <= 5 * 128, "a symbol's copies");
+        uint4 *dst = reinterpret_cast<uint4 *>(in) + tl;
+        const uint8_t *src = iq + b0a + 16 * tl;
+        const bool head = b0a < 0;
+#pragma unroll
+        for (int i = 0; i < 5; i++) {
+            if (i == 4 && tl + 4 * 128 >= nvec) break;
+            if (!head || b0a + 16 * (tl + 128 * i) >= 0) {
 #if defined(NB_EMU)
-                dst[v] = *reinterpret_cast<const uint4 *>(iq + a);
+                dst[128 * i] = *reinterpret_cast<const uint4 *>(src + 2048 * i);
 #else
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst + v)), "l"(iq + a) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst + 128 * i)), "l"(src + 2048 * i) : "memory");
 #endif
             } else {
-                dst[v] = make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);      // before the stream's first sample
+                dst[128 * i] = make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);   // before the stream's first sample
             }
         }
 #if !defined(NB_EMU)
@@ -761,15 +767,17 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
     // kept bins (sync.c:785-789, fftshift defines.h:123-138): with q = tl + 128 h and natural bin k = q + 256 k3,
     //   k3 = 5 (q >= 222) -> compact q - 222,  k3 = 6 (q <= 232) -> q + 34      (lower sideband, bins 478..744)
     //   k3 = 1 (q >= 24)  -> compact q + 243,  k3 = 2 (q <= 34)  -> q + 499     (upper sideband, bins 1304..1570)
-    // The reference carriers also go to zref[sym]: bit 4 h + k of ref_mask[tl] marks the thread's k-th store of round h
-    // as one, ref_slot gives its slot.  (Tables rather than arithmetic on q: per-thread constants would be hoisted out
-    // of the symbol loop and spilled.)
+    // The reference carriers also go to zref[sym].  A thread makes at most one such store: ref_plan[tl] holds its index
+    // 4 h + k (the k-th store of round h) in bits 5-7 and its slot in bits 0-4, or 0xff for none (store 7 never
+    // happens: q = tl + 128 > 34).  So each store costs one compare and a predicated shared store.  (A table rather
+    // than arithmetic on q: per-thread constants would be hoisted out of the symbol loop and spilled.)
     float2 *dst = p.bins + ((size_t)s * BLK + sym) * NBINS;
-    float2 *zr = zref[sym];
-    const unsigned mask = ref_mask[tl];
-    auto put = [&](int c, float2 v, int bit) {
+    const unsigned plan = ref_plan[tl];
+    float2 *zp = zref[sym] + (plan & 31u);
+    const unsigned pk = plan >> 5;
+    auto put = [&](int c, float2 v, unsigned k) {
         dst[c] = v;
-        if (mask & (1u << bit)) zr[ref_slot[c]] = v;
+        if (pk == k) *zp = v;
     };
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -1471,17 +1479,19 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
     const int s = (int)blockIdx.x / C, rank = (int)blockIdx.x % C;
     StreamState &st = p.st[s];
     for (int i = t; i < FFT_TW; i += FRONT_THREADS) sm.tw[i] = __ldg(&p.twid[i]);
-    for (int c = t; c < NBINS; c += FRONT_THREADS)     // lower slot i: compact 19 i; upper slot MAXREF + i: 533 - 19 i
-        sm.ref_slot[c] = c < SIDE ? (c % PW == 0 ? c / PW : -1) : ((NBINS - 1 - c) % PW == 0 ? MAXREF + (NBINS - 1 - c) / PW : -1);
     if (t < 128) {                                     // front_demod's stores of thread t: compact q-222, q+34, q+243, q+499
-        unsigned m = 0;
+        unsigned m = 0xffu;                            // lower slot i: compact 19 i; upper slot MAXREF + i: 533 - 19 i
         for (int h = 0; h < 2; h++) {
             const int q = t + 128 * h;
             const int c[4] = { q >= 222 ? q - 222 : -1, q <= 232 ? q + 34 : -1, q >= 24 ? q + 243 : -1, q <= 34 ? q + 499 : -1 };
-            for (int k = 0; k < 4; k++)
-                if (c[k] >= 0 && (c[k] < SIDE ? c[k] % PW == 0 : (NBINS - 1 - c[k]) % PW == 0)) m |= 1u << (4 * h + k);
+            for (int k = 0; k < 4; k++) {
+                if (c[k] < 0) continue;
+                const int slot = c[k] < SIDE ? (c[k] % PW == 0 ? c[k] / PW : -1)
+                                             : ((NBINS - 1 - c[k]) % PW == 0 ? MAXREF + (NBINS - 1 - c[k]) / PW : -1);
+                if (slot >= 0) m = (unsigned)(4 * h + k) << 5 | (unsigned)slot;   // (at most one per thread)
+            }
         }
-        sm.ref_mask[t] = (uint8_t)m;
+        sm.ref_plan[t] = (uint8_t)m;
     }
     __syncthreads();
 
@@ -1545,7 +1555,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         }
 #pragma unroll 1
         for (int pass = 0; pass < BLK / (TEAMS * C); pass++)
-            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.tw, sm.zref, sm.ref_slot, sm.ref_mask, team, tl, start, samperr, theta, phase0);
+            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.tw, sm.zref, sm.ref_plan, team, tl, start, samperr, theta, phase0);
         if (CL) {
             __threadfence();
             cluster_barrier();                        // every CTA's bins are in L2
