@@ -276,7 +276,8 @@ int nrsc5b_fft2048(int device, const float *in, float *out, int nffts);
 typedef struct nrsc5b_channelizer nrsc5b_channelizer_t;
 int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch);
 void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c);
-/* taps[nch][256][2] (real, imaginary part of W_k[u]) and phasor[11907][2]; either may be NULL */
+/* taps[nch][256][2] (real, imaginary part of W_k[u]; an AM-plan handle: [nch][512][2]) and phasor[11907][2]; either
+ * may be NULL */
 int nrsc5b_chan_tables(nrsc5b_channelizer_t *c, int16_t *taps, int16_t *phasor);
 /* the same tables computed on the host without a device (the definition's inputs, for the numpy restatement) */
 int nrsc5b_chan_make_tables(const int *offsets_100khz, int nch, int16_t *taps, int16_t *phasor);
@@ -332,6 +333,39 @@ int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *d_cs16, siz
 int nrsc5b_chan_push_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, void *d_out, size_t out_stride,
                           void *cuda_stream, long long *nout);
 int nrsc5b_chan_feed_cs16(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e, const int *streams, const int16_t *cs16, size_t nvalues);
+
+/* AM band plan: one cu8 or cs16 capture at 32 x 46 511.71875 = 1 488 375 S/s - the rate the reference asks of an AM
+ * device; it spans +-744 kHz, the whole medium-wave band - -> `nch` AM channels at 46 511.71875 S/s cs16, the format an
+ * NRSC5B_MODE_AM engine created with input_cs16 = 1 takes.  Channel k is centred `offsets_10khz[k]` x 10 kHz from the
+ * capture's centre; offsets beyond +-74 are outside the capture: NRSC5B_EINVAL.  10 kHz / 1 488 375 Hz = 80 / 11907, so
+ * the phasor table P is the FM plan's; the filter has 512 taps (h_am: Kaiser-windowed sinc, -6 dB at 23 kHz, beta 8.8,
+ * unit DC gain; the integer taps of channel 0 are within +-0.001 dB up to 15 kHz and 87.1 dB down from 31.5 kHz on,
+ * where the stations that alias onto a channel after the decimation by 32 begin).  Integer-exact definition:
+ *     W_k[u]  = round(2^19 h_am[511-u] conj(P[(80 m_k u) mod 11907]) / 32767)
+ *     cu8:   acc = sum_{u<512} W_k[u] (x[32 n + u] - (127+127j));  v = (acc + 2^12) >> 13
+ *     cs16:  acc = sum_{u<512} W_k[u]  x[32 n + u];                v = sat16((acc + 2^18) >> 19)
+ *     y[k][n] = sat16((v conj(P[(2560 m_k n) mod 11907]) + 2^14) >> 15)
+ *     N_am(T) = T >= 512 ? (T - 512) / 32 + 1 : 0;   carry = the samples from 32 N_am(T) on (at most 511 samples:
+ *     1022 bytes of cu8, 2044 of cs16)
+ * The cu8 gain is 64 output LSB per input LSB, as in the FM plan (the reference's own AM cu8 path has 128; the AM
+ * receiver normalises on its carrier and training symbols).  For x16 = 64 (x8 - 127) the cs16 output equals the cu8
+ * output bit for bit.
+ * The plan is fixed at create, like the sample format.  Every other entry point (nrsc5b_chan_run*, _push*, _feed*,
+ * _tables, _reset, _destroy) is shared and behaves as documented above with 512 taps and N_am(T): nrsc5b_chan_tables
+ * returns taps[nch][512][2], and nrsc5b_chan_feed* takes exactly an NRSC5B_MODE_AM engine with input_cs16 = 1 that reads
+ * its own buffers (an FM handle on an AM engine, an AM handle on an FM engine, an AM engine created for cu8 input:
+ * NRSC5B_EINVAL, nothing changed).
+ * A stream fed from a channel that holds exact zeros (a digitally silent channel of a synthetic capture) behaves as
+ * the reference does on such input: its carrier regression divides by the previous symbol's centre bin (reference
+ * src/acquire.c:199-201) and stays NaN from then on; nrsc5b_reset(e, stream) recovers it.  A real capture's noise
+ * floor keeps clear of that. */
+int nrsc5b_chan_create_am(nrsc5b_channelizer_t **out, int device, const int *offsets_10khz, int nch);
+int nrsc5b_chan_create_am_cs16(nrsc5b_channelizer_t **out, int device, const int *offsets_10khz, int nch);
+/* the AM plan's tables without a device: taps[nch][512][2], phasor[11907][2] (the FM table); either may be NULL */
+int nrsc5b_chan_make_tables_am(const int *offsets_10khz, int nch, int16_t *taps, int16_t *phasor);
+/* output samples per channel of an AM-plan capture of nbytes (cu8; cs16: int16 values): nbytes / 64 - 15 for
+ * nbytes % 64 == 0 */
+long long nrsc5b_chan_outputs_am(size_t nbytes);
 
 const char *nrsc5b_version(void);
 

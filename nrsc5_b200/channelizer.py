@@ -1,5 +1,6 @@
 """ctypes binding of the wideband channeliser (include/nrsc5_b200.h, csrc/channelizer.cu): one cu8 or cs16 capture at
-23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take.
+23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take; or, with
+band="am", one capture at 1 488 375 S/s -> AM channels (10 kHz grid) at 46 511.71875 S/s cs16 through a 512-tap bank.
 No CPU fallback: constructing a Channelizer without a CUDA device raises."""
 from __future__ import annotations
 
@@ -10,7 +11,17 @@ import numpy as np
 from .engine import EngineError, _check, load_library
 
 WIDE_RATE = 23814000.0          # 32 x 744 187.5
+AM_WIDE_RATE = 1488375.0        # 32 x 46 511.71875
 TAPS, PERIOD, DECIM = 256, 11907, 32
+TAPS_AM = 512
+# band plan -> (taps per channel, suffix of the plan's own entry points)
+_BANDS = {"fm": (TAPS, ""), "am": (TAPS_AM, "_am")}
+
+
+def _band(band):
+    if band not in _BANDS:
+        raise ValueError(f"band: {band!r} is neither 'fm' nor 'am'")
+    return _BANDS[band]
 
 
 def _lib():
@@ -34,44 +45,57 @@ def _lib():
         L.nrsc5b_chan_run_cs16.argtypes = [vp, vp, sz, vp]
         L.nrsc5b_chan_push_cs16.argtypes = [vp, vp, sz, vp, sz, vp, ctypes.POINTER(ctypes.c_longlong)]
         L.nrsc5b_chan_feed_cs16.argtypes = [vp, vp, vp, vp, sz]
+        L.nrsc5b_chan_create_am.argtypes = [ctypes.POINTER(vp), ci, vp, ci]
+        L.nrsc5b_chan_create_am_cs16.argtypes = [ctypes.POINTER(vp), ci, vp, ci]
+        L.nrsc5b_chan_make_tables_am.argtypes = [vp, ci, vp, vp]
+        L.nrsc5b_chan_outputs_am.argtypes = [sz]
+        L.nrsc5b_chan_outputs_am.restype = ctypes.c_longlong
         L._chan_ready = True
     return L
 
 
-def stream_outputs(pushed: int, nbytes: int) -> int:
+def stream_outputs(pushed: int, nbytes: int, band: str = "fm") -> int:
     """Outputs per channel a push of nbytes (cu8; cs16: int16 values) emits after `pushed` complex samples
-    (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0."""
+    (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0 (band "am": 512 for 256)."""
+    ntaps = _band(band)[0]
+
     def n(t):
-        return (t - TAPS) // DECIM + 1 if t >= TAPS else 0
+        return (t - ntaps) // DECIM + 1 if t >= ntaps else 0
     return n(pushed + nbytes // 2) - n(pushed)
 
 
-def make_tables(offsets_100khz):
-    """The integer tables of the definition, computed on the host (no device): taps[nch][256][2], phasor[11907][2]."""
+def make_tables(offsets_100khz, band: str = "fm"):
+    """The integer tables of the definition, computed on the host (no device): taps[nch][256][2], phasor[11907][2]
+    (band "am": offsets in 10 kHz steps, taps[nch][512][2])."""
+    ntaps, sfx = _band(band)
     off = np.ascontiguousarray(offsets_100khz, dtype=np.int32)
-    taps = np.empty((off.size, TAPS, 2), dtype=np.int16)
+    taps = np.empty((off.size, ntaps, 2), dtype=np.int16)
     ph = np.empty((PERIOD, 2), dtype=np.int16)
-    _check(_lib().nrsc5b_chan_make_tables(off.ctypes.data, off.size, taps.ctypes.data, ph.ctypes.data), "nrsc5b_chan_make_tables")
+    name = "nrsc5b_chan_make_tables" + sfx
+    _check(getattr(_lib(), name)(off.ctypes.data, off.size, taps.ctypes.data, ph.ctypes.data), name)
     return taps, ph
 
 
-def outputs(nbytes: int) -> int:
+def outputs(nbytes: int, band: str = "fm") -> int:
     """Outputs per channel of a capture of nbytes cu8 bytes (or as many int16 values of cs16)."""
-    return int(_lib().nrsc5b_chan_outputs(nbytes & ~63))
+    return int(getattr(_lib(), "nrsc5b_chan_outputs" + _band(band)[1])(nbytes & ~63))
 
 
 class Channelizer:
     """input_cs16=False: the capture is cu8 (uint8, lengths in bytes); True: cs16 (int16, lengths in int16 values,
-    the _cs16 entry points).  Either way two input units make one complex sample."""
-    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False):
+    the _cs16 entry points).  Either way two input units make one complex sample.  band="am": the AM plan (offsets in
+    10 kHz steps of a 1 488 375 S/s capture, 512 taps); only create differs, every other call is the handle's."""
+    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False, band: str = "fm"):
         self._L = _lib()
+        self.band = band
+        self.taps = _band(band)[0]
         self.offsets = np.ascontiguousarray(offsets_100khz, dtype=np.int32)
         self.nch = int(self.offsets.size)
         self.input_cs16 = bool(input_cs16)
         self._dtype = np.int16 if self.input_cs16 else np.uint8
         self._sfx = "_cs16" if self.input_cs16 else ""
         self._h = ctypes.c_void_p()
-        name = "nrsc5b_chan_create" + self._sfx
+        name = "nrsc5b_chan_create" + _band(band)[1] + self._sfx
         _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), name)
         self.device = device
         self.pushed = 0                 # T: complex samples pushed since create / reset (mirrors the handle's count)
@@ -94,7 +118,7 @@ class Channelizer:
             pass
 
     def tables(self):
-        taps = np.empty((self.nch, TAPS, 2), dtype=np.int16)
+        taps = np.empty((self.nch, self.taps, 2), dtype=np.int16)
         ph = np.empty((PERIOD, 2), dtype=np.int16)
         _check(self._L.nrsc5b_chan_tables(self._h, taps.ctypes.data, ph.ctypes.data), "nrsc5b_chan_tables")
         return taps, ph
@@ -107,7 +131,7 @@ class Channelizer:
         """Host capture (uint8, or int16 with input_cs16; I/Q interleaved) -> int16 array [nch][2 * outputs] (I, Q
         interleaved)."""
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
-        n = outputs(a.size)
+        n = outputs(a.size, self.band)
         out = np.empty((self.nch, 2 * max(n, 0)), dtype=np.int16)
         if n > 0:
             self._call("nrsc5b_chan_run", self._h, a.ctypes.data, a.size, out.ctypes.data)
@@ -138,7 +162,7 @@ class Channelizer:
         [nch][2 * n]: the outputs it completes.  Synchronous."""
         import torch
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
-        n = stream_outputs(self.pushed, a.size)
+        n = stream_outputs(self.pushed, a.size, self.band)
         dev = torch.device("cuda", self.device)
         out = torch.empty((self.nch, 2 * max(n, 1)), dtype=torch.int16, device=dev)
         stream = torch.cuda.current_stream(dev)
@@ -149,7 +173,7 @@ class Channelizer:
 
     def feed(self, engine, data, streams=None):
         """The next piece of the capture -> channel k appended to cs16 stream streams[k] of `engine` (an Engine made
-        with input_cs16=True; streams None: stream k).  data: a uint8 (input_cs16: int16) numpy array or (pointer, nbytes
+        with input_cs16=True and the band's mode; streams None: stream k).  data: a uint8 (input_cs16: int16) numpy array or (pointer, nbytes
         or int16 values) to host or device memory.  Raises EngineError on NRSC5B_EFULL (nothing taken: process() and feed the same data again)."""
         if isinstance(data, tuple):
             ptr, nbytes = int(data[0]), int(data[1])

@@ -45,6 +45,29 @@
 // x_hi plane (wgmma s8 x s8) to A1 = sum W x_hi (|A1| < 2^28) in 32 registers, then the x_lo plane (wgmma u8 x s8)
 // to A2 = sum W x_lo (|A2| < 2^29) in the 64 accumulators, and combines acc = 256 A1 + A2 in exact 32-bit pieces
 // before the shared epilogue.  A tile's two planes take two consecutive stages of the ring.
+//
+// AM band plan (nrsc5b_chan_create_am*): one capture at 32 x 46 511.71875 = 1 488 375 S/s, the rate the reference asks
+// of an AM device, spans +-744 kHz - the whole medium-wave band - and goes to 10 kHz channels at 46 511.71875 S/s cs16,
+// what an AM engine reads.  10 kHz / 1 488 375 Hz = 80 / 11907: the same phasor table P.  m_k = the offset in 10 kHz
+// steps, |m_k| <= 74:
+//
+//     W_k[u]  = round(2^19 h_am[511-u] conj(P[(80 m_k u) mod 11907]) / 32767)            u < 512
+//     cu8:   acc = sum_{u<512} W_k[u] (x[32 n + u] - (127+127j));  v = (acc + 2^12) >> 13
+//     cs16:  acc = sum_{u<512} W_k[u]  x[32 n + u];                v = sat16((acc + 2^18) >> 19)
+//     y[k][n] = sat16((v conj(P[(2560 m_k n) mod 11907]) + 2^14) >> 15)
+//     N_am(T) = T >= 512 ? (T - 512) / 32 + 1 : 0;   carry = the samples from 32 N_am(T) on (<= 511 samples)
+//
+// h_am: 512-tap Kaiser-windowed sinc (-6 dB at 23 kHz, beta 8.8), unit DC gain.  Measured on the integer taps of
+// channel 0: within +-0.001 dB up to 15 kHz, 87.1 dB down from 31.5 kHz on (tests/test_channelizer_am.py holds them to
+// +-0.25 dB and 80 dB).  FM's 256 taps would give about 48 dB there, and in a hybrid AM signal the digital carriers sit
+// 30 - 50 dB under an analog carrier, the aliases of the stations k x 46.5 kHz away a few kHz off centre, on top of them.
+// The tap scale stays 2^19 (the bounds are re-derived at make_tables), the cu8 gain 64 output LSB per input LSB.
+// In the kernel the second 256 taps are the same GEMM on capture-matrix rows 8 further on: KPASS = 2 passes of K = 512
+// into the same accumulators (16 TMA boxes and 32 wgmmas per tile and plane).  Shared memory: both tap halves resident
+// (131 072 B) + two 32 KB stages (65 536 B), one per consumer warpgroup, which a tile's passes and planes go through
+// one after the other + alignment, barriers and epilogue tables (25 744 B) = 222 352 B, the same total as the FM
+// instantiation's 64 KB of taps + four stages.  A consumer's loads and wgmmas therefore alternate; what overlaps is
+// the other consumer's loads, wgmmas and epilogue.  The input is 1/16 of the FM rate: residency, not speed, is the limit.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -60,27 +83,38 @@
 
 namespace nbch {
 
-constexpr int DECIM = 32, TAPS = 256, KBYTES = 2 * TAPS;          // 512 bytes of K per output row
-constexpr int CHUNK = 64, NCHUNK = KBYTES / CHUNK;               // K chunks of 64 bytes (one capture-matrix row each)
+constexpr int DECIM = 32, PASS_TAPS = 256, KBYTES = 2 * PASS_TAPS; // one pass: 256 taps, 512 bytes of K per output row (FM: one pass, AM: two)
+constexpr int CHUNK = 64, NCHUNK = KBYTES / CHUNK;               // K chunks of 64 bytes (one capture-matrix row each) per pass
 constexpr int TILE_M = 64;                                        // output samples per tile (one warpgroup's wgmma M)
 constexpr int GROUP = 32, TILE_N = 4 * GROUP;                    // channels per CTA, rows of B
 constexpr int PERIOD = 11907;                                     // phasor table length (100 kHz / 23.814 MHz = 50 / 11907)
 constexpr int SHIFT1 = 13, TAP_SCALE_LOG2 = 19;                   // unit DC gain -> 64 LSB per input LSB (the cu8 -> Q15 convention);
                                                                   // taps stay below 127 * 256 + 127: both bytes of the split are int8
 constexpr int THREADS = 384;                                      // producer warpgroup + two consumer warpgroups
-constexpr int STAGES = 4;
-constexpr uint32_t A_STAGE_BYTES = NCHUNK * TILE_M * CHUNK;      // 32768
-constexpr uint32_t W_BYTES = NCHUNK * TILE_N * CHUNK;            // 65536
+constexpr int STAGES = 4;                                         // most capture stages a ring has (the barriers are laid out for it)
+constexpr uint32_t A_STAGE_BYTES = NCHUNK * TILE_M * CHUNK;      // 32768: one pass of one plane of a tile
+constexpr uint32_t W_BYTES = NCHUNK * TILE_N * CHUNK;            // 65536: one pass of a group's taps
 constexpr int HALF = PERIOD / 2 + 1;                              // phasor table entries 0 .. 5953; the rest are their conjugates
 // half table, rotation steps, offset corrections, destination offsets
 constexpr uint32_t EPI_BYTES = ((HALF * 4 + 15) & ~15) + GROUP * 4 + 2 * GROUP * 4 + GROUP * 8;
-constexpr uint32_t SMEM_BYTES = W_BYTES + STAGES * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
-static_assert(SMEM_BYTES <= 227 * 1024, "more shared memory than an H100 block may have");
+// KPASS = 1 (256 taps): 64 KB of taps + four stages = 222 352 B.  KPASS = 2 (512 taps): both tap halves stay resident
+// (128 KB), which leaves room for a ring of two stages - again 222 352 B - that a tile's passes and planes go through
+// one after the other.
+constexpr int stages_of(int kpass) { return kpass == 1 ? STAGES : 2; }
+constexpr uint32_t smem_bytes(int kpass)
+{
+    return kpass * W_BYTES + stages_of(kpass) * A_STAGE_BYTES + 1024 /* alignment */ + 256 /* barriers */ + EPI_BYTES;
+}
+static_assert(smem_bytes(1) <= 227 * 1024 && smem_bytes(2) <= 227 * 1024, "more shared memory than an H100 block may have");
 // cs16: the byte planes of up to PLANE_SAMPLES samples, x_hi rows first, then x_lo rows (one TMA map over both)
 constexpr long long PLANE_SAMPLES = (1ll << 22) + 256;
 constexpr int PLANE_ROWS = (int)(2 * PLANE_SAMPLES / CHUNK);
-constexpr long long PIECE_OUT = 1ll << 17;                        // outputs per launch of the one-shot cs16 entry: 32 n + 224 <= PLANE_SAMPLES
-static_assert(DECIM * PIECE_OUT + TAPS - DECIM <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
+// outputs per launch of the one-shot cs16 entry: 32 n + taps - 32 <= PLANE_SAMPLES (2^17 with 256 taps, 2^17 - 7 with 512)
+constexpr long long piece_out(int taps)
+{
+    return (PLANE_SAMPLES - taps) / DECIM + 1 < (1ll << 17) ? (PLANE_SAMPLES - taps) / DECIM + 1 : 1ll << 17;
+}
+static_assert(piece_out(256) == 1ll << 17 && DECIM * piece_out(512) + 512 - DECIM <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
 
 struct Params {
     int nch;                   // channels
@@ -91,7 +125,7 @@ struct Params {
     int16_t *out;              // cs16 (I, Q interleaved): output n of channel k goes to out + dst[k] + 2 n
     const long long *dst;      // [nch] int16 offsets of each channel's output 0; null: dst[k] = k * out_stride
     size_t out_stride;
-    const int *rot_step;       // [nch] (1600 m_k) mod 11907
+    const int *rot_step;       // [nch] (1600 m_k) mod 11907 (AM plan: 2560 m_k)
     const long long *corr;     // [nch][2] 127 * (sum Wr - sum Wi), 127 * (sum Wi + sum Wr)   (already in acc units)
     const short2 *phasor;      // [PERIOD]
 };
@@ -187,20 +221,35 @@ struct Barriers {
     uint64_t w_full, a_full[STAGES], a_empty[STAGES];
 };
 
-// CS16: map_x addresses the two byte planes of a cs16 capture, the x_lo plane PLANE_ROWS rows after the x_hi plane
-template <bool CS16>
+// The ring: unit `it` of a CTA's sequence (a tile's U = PLANES * KPASS stages in a row, the tiles going to the two
+// consumers in turn) lands in stage ring_stage(it), which has been filled ring_use(it) times before.  A thread may only
+// wait for a barrier phase if it has seen the one before (a wait for the parity of a phase that has not begun passes at
+// once), so a stage is only ever read by one consumer.  KPASS = 1: four stages taken round robin - U divides 2, so
+// consumer w gets stages w, w + 2 (cu8) or 2 w, 2 w + 1 (cs16).  KPASS = 2: two stages, stage w is consumer w's, and
+// its units pass through it one at a time.
+template <int U, int KPASS>
+__device__ __forceinline__ int ring_stage(unsigned it) { return KPASS == 1 ? it % STAGES : (it / U) & 1; }
+template <int U, int KPASS>
+__device__ __forceinline__ unsigned ring_use(unsigned it) { return KPASS == 1 ? it / STAGES : (it / (2 * U)) * U + it % U; }
+
+// CS16: map_x addresses the two byte planes of a cs16 capture, the x_lo plane PLANE_ROWS rows after the x_hi plane.
+// KPASS: K = 512 passes per output row (256 taps each).  Pass ps of output n reads capture-matrix rows n + 8 ps ..
+// n + 8 ps + 7 against tap chunks 8 ps .. 8 ps + 7 and adds into the same accumulators, so a 512-tap tile is two
+// stages of the ring per plane; with cs16 the x_hi plane is folded into A1 after all its passes, then the x_lo plane runs.
+template <bool CS16, int KPASS>
 __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                                                            Params p)
 {
-    constexpr int PLANES = CS16 ? 2 : 1;                           // capture stages per tile
+    constexpr int PLANES = CS16 ? 2 : 1;                           // a tile takes PLANES * KPASS capture stages
+    constexpr int NST = stages_of(KPASS), WB = KPASS * (int)W_BYTES, U = PLANES * KPASS;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t *smem_w = smem;                                        // [8 chunks][128 rows][64 B]
-    uint8_t *smem_a = smem + W_BYTES;                              // [STAGES][8 chunks][64 rows][64 B]
-    Barriers &bar = *reinterpret_cast<Barriers *>(smem + W_BYTES + STAGES * A_STAGE_BYTES);
+    uint8_t *smem_w = smem;                                        // [KPASS * 8 chunks][128 rows][64 B]
+    uint8_t *smem_a = smem + WB;                                   // [NST][8 chunks][64 rows][64 B]
+    Barriers &bar = *reinterpret_cast<Barriers *>(smem + WB + NST * A_STAGE_BYTES);
     // the epilogue's tables in shared memory: the first half of the phasor table (P[11907 - i] = conj(P[i]), made so on
     // the host), and this group's rotation steps, offset corrections and output destinations
-    short2 *ph_half = reinterpret_cast<short2 *>(smem + W_BYTES + STAGES * A_STAGE_BYTES + 256);
+    short2 *ph_half = reinterpret_cast<short2 *>(smem + WB + NST * A_STAGE_BYTES + 256);
     int *s_rot = reinterpret_cast<int *>(reinterpret_cast<uint8_t *>(ph_half) + ((HALF * 4 + 15) & ~15));
     uint32_t *s_corr = reinterpret_cast<uint32_t *>(s_rot + GROUP);
     long long *s_dst = reinterpret_cast<long long *>(s_corr + 2 * GROUP);
@@ -217,7 +266,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     }
     if (threadIdx.x == 0) {
         mbar_init(&bar.w_full, 1);
-        for (int i = 0; i < STAGES; i++) {
+        for (int i = 0; i < NST; i++) {
             mbar_init(&bar.a_full[i], 1);
             mbar_init(&bar.a_empty[i], 4);                         // one arrival per warp of the consuming warpgroup
         }
@@ -229,18 +278,19 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
     if (wgi == 0) {
         // ===== TMA producer (one thread) =====
         if (threadIdx.x == 0) {
-            mbar_expect_tx(&bar.w_full, W_BYTES);
-            for (int c = 0; c < NCHUNK; c++)
-                tma_load_2d(smem_w + (size_t)c * TILE_N * CHUNK, &map_w, &bar.w_full, 0, (group * NCHUNK + c) * TILE_N);
+            mbar_expect_tx(&bar.w_full, WB);
+            for (int c = 0; c < KPASS * NCHUNK; c++)
+                tma_load_2d(smem_w + (size_t)c * TILE_N * CHUNK, &map_w, &bar.w_full, 0, (group * KPASS * NCHUNK + c) * TILE_N);
             unsigned it = 0;
             for (long long tile = slot; tile < p.tiles; tile += nslots)
-                for (int pl = 0; pl < PLANES; pl++, it++) {      // cs16: the x_hi plane, then the x_lo plane
-                    const int s = it % STAGES;
-                    if (it >= STAGES) mbar_wait(&bar.a_empty[s], (it / STAGES - 1) & 1);
+                for (int pp = 0; pp < PLANES * KPASS; pp++, it++) {   // cs16: the x_hi plane's passes, then the x_lo plane's
+                    const int pl = pp / KPASS, ps = pp % KPASS;
+                    const int s = ring_stage<U, KPASS>(it);
+                    if (KPASS == 1 ? it >= STAGES : ring_use<U, KPASS>(it) > 0) mbar_wait(&bar.a_empty[s], (ring_use<U, KPASS>(it) - 1) & 1);
                     mbar_expect_tx(&bar.a_full[s], A_STAGE_BYTES);
-                    for (int c = 0; c < NCHUNK; c++)             // K chunk c of output row n = capture-matrix row n + c
+                    for (int c = 0; c < NCHUNK; c++)             // K chunk c of pass ps of output row n = capture-matrix row n + 8 ps + c
                         tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, &map_x, &bar.a_full[s], 0,
-                                    (int)(tile * TILE_M) + c + pl * PLANE_ROWS);
+                                    (int)(tile * TILE_M) + ps * NCHUNK + c + pl * PLANE_ROWS);
                 }
         }
         return;
@@ -252,26 +302,29 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
 #pragma unroll
     for (int i = 0; i < 8; i++) row[i] = p.out + s_dst[4 * i + q];
     mbar_wait(&bar.w_full, 0);
-    unsigned it = (unsigned)wg * PLANES;
-    for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2 * PLANES) {
+    unsigned it = (unsigned)wg * PLANES * KPASS;
+    for (long long tile = slot + (long long)wg * nslots; tile < p.tiles; tile += 2ll * nslots, it += 2 * PLANES * KPASS) {
         uint32_t d[64];                                            // (the first wgmma overwrites it: accumulate = 0)
         int a1[32];                                                // cs16: A1 = sum W x_hi, [channel i][row h][re, im]
         if constexpr (CS16) {
-            const int s = it % STAGES;
-            mbar_wait(&bar.a_full[s], (it / STAGES) & 1);
-            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll 1
+            for (int ps = 0; ps < KPASS; ps++) {
+                const int s = ring_stage<U, KPASS>(it + ps);
+                mbar_wait(&bar.a_full[s], ring_use<U, KPASS>(it + ps) & 1);
+                asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-            for (int c = 0; c < NCHUNK; c++)
+                for (int c = 0; c < NCHUNK; c++)
 #pragma unroll
-                for (int k = 0; k < CHUNK / 32; k++) {
-                    const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
-                    const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)c * TILE_N * CHUNK, 32u * k);
-                    wgmma_s8s8(d, da, db, (c | k) ? 1u : 0u);
-                }
-            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar.a_empty[s]);
+                    for (int k = 0; k < CHUNK / 32; k++) {
+                        const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
+                        const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)(ps * NCHUNK + c) * TILE_N * CHUNK, 32u * k);
+                        wgmma_s8s8(d, da, db, (ps | c | k) ? 1u : 0u);
+                    }
+                asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+                asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bar.a_empty[s]);
+            }
             // |A1| <= 128 sum(|Wr| + |Wi|) < 2^28: the wrapped 32-bit 256 hi + lo is the value
 #pragma unroll
             for (int i = 0; i < 8; i++)
@@ -281,22 +334,25 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
                     a1[4 * i + 2 * h + 1] = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h]);
                 }
         }
-        const unsigned il = it + PLANES - 1;                       // the stage of the unsigned operand (cu8: the capture; cs16: x_lo)
-        const int s = il % STAGES;
-        mbar_wait(&bar.a_full[s], (il / STAGES) & 1);
-        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll 1
+        for (int ps = 0; ps < KPASS; ps++) {
+            const unsigned il = it + (PLANES - 1) * KPASS + ps;    // the stage of the unsigned operand (cu8: the capture; cs16: x_lo)
+            const int s = ring_stage<U, KPASS>(il);
+            mbar_wait(&bar.a_full[s], ring_use<U, KPASS>(il) & 1);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-        for (int c = 0; c < NCHUNK; c++)
+            for (int c = 0; c < NCHUNK; c++)
 #pragma unroll
-            for (int k = 0; k < CHUNK / 32; k++) {                 // wgmma K = 32 bytes
-                const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
-                const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)c * TILE_N * CHUNK, 32u * k);
-                wgmma_u8s8(d, da, db, (c | k) ? 1u : 0u);
-            }
-        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar.a_empty[s]);               // the stage's bytes are no longer needed
+                for (int k = 0; k < CHUNK / 32; k++) {             // wgmma K = 32 bytes
+                    const uint64_t da = wgmma_desc_sw64(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, 32u * k);
+                    const uint64_t db = wgmma_desc_sw64(smem_w + (size_t)(ps * NCHUNK + c) * TILE_N * CHUNK, 32u * k);
+                    wgmma_u8s8(d, da, db, (ps | c | k) ? 1u : 0u);
+                }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bar.a_empty[s]);           // the stage's bytes are no longer needed
+        }
 
         // ===== epilogue: rows 16 wwarp + lane / 4 (h = 0) and + 8 (h = 1) of the tile =====
         // 32-bit arithmetic throughout: 256 * hi + lo wraps, the filter output itself is bounded by
@@ -364,8 +420,8 @@ __global__ void k_split_cs16(const int16_t *__restrict__ src, long long nvalues,
 }
 
 // Streaming: after a launch over the staging buffer has used the outputs it could, the samples from 32 x (outputs) on -
-// at most 255 samples, 510 bytes of cu8 or 1020 of cs16 - move to the front of the buffer, where the next push's bytes
-// are appended to them.  Source and destination can overlap: one block (of nbytes / 2 threads or more) reads everything
+// at most taps - 1 samples: 510 bytes of cu8 or 1020 of cs16 with 256 taps, 1022 or 2044 with 512 - move to the front
+// of the buffer, where the next push's bytes are appended to them.  Source and destination can overlap: one block (of nbytes / 2 threads or more) reads everything
 // before it writes.
 __global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
 {
@@ -376,7 +432,7 @@ __global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
     if (i < nbytes) *reinterpret_cast<uint16_t *>(buf + i) = v;
 }
 
-constexpr size_t STAGE_CAP = (4u << 20) + 512;                    // cu8 staging: the carry (< 512 bytes) + 4 MiB of new capture
+constexpr size_t stage_cap_cu8(int taps) { return (4u << 20) + 2 * (size_t)taps; }   // cu8 staging: the carry (< 2 taps bytes) + 4 MiB of new capture
 constexpr size_t STAGE_CAP_CS16 = 4 * PLANE_SAMPLES;              // cs16 staging: as many samples as the planes hold (16 MiB + 1 KiB)
 constexpr int DST_RING = 8;                                       // destination tables in flight (nrsc5b_chan_feed)
 
@@ -387,13 +443,33 @@ constexpr int DST_RING = 8;                                       // destination
 // ===========================================================================
 using namespace nbch;
 
+// A band plan: everything that differs between the FM grid (100 kHz channels of a 23 814 000 S/s capture) and the AM
+// grid (10 kHz channels of a 1 488 375 S/s capture).  Both decimate by 32 and share the 11907-entry phasor table:
+// 100 kHz / 23.814 MHz = 50 / 11907, 10 kHz / 1 488 375 Hz = 80 / 11907; the mixer steps are 32 x those.
+struct Plan {
+    int taps;                             // per channel: KPASS = taps / 256 passes of the kernel
+    int tap_step, mix_step;               // phasor steps per input sample in W_k, per output sample in the mixer
+    double fc, beta;                      // prototype: Kaiser-windowed sinc, -6 dB at fc (cycles per input sample)
+    int max_offset;                       // |m_k| the capture holds (0: not limited)
+    int engine_mode;                      // the engine nrsc5b_chan_feed may write into
+};
+// FM: -6 dB at 372 kHz: flat over a hybrid FM channel (+-200 kHz), >= 55 dB down from 544 kHz on (what folds onto the
+// channel after /32)
+static const Plan PLAN_FM = { 256, 50, 1600, 372000.0 / 23814000.0, 5.65, 0, NRSC5B_MODE_FM };
+// AM: -6 dB at 23 kHz.  The integer taps of channel 0 are within +-0.001 dB up to 15 kHz (a hybrid AM channel) and
+// 87.1 dB down from 31.5 kHz on: what folds onto a channel after /32 are the stations k x 46.5 kHz away, which on the
+// 10 kHz grid land a few kHz off centre, on carriers 30 - 50 dB below an analog host.  The capture spans +-744 kHz:
+// offsets beyond +-74 are not in it.
+static const Plan PLAN_AM = { 512, 80, 2560, 23000.0 / 1488375.0, 8.8, 74, NRSC5B_MODE_AM };
+
 struct nrsc5b_channelizer {
     int device, nch, ngroups;
+    const Plan *plan;                     // the band plan, fixed at create
     bool cs16;                            // the input format, fixed at create
-    std::vector<int> offsets;             // m_k: channel offset from the capture centre in 100 kHz steps
-    std::vector<int16_t> taps;            // [nch][TAPS][2] (Wr, Wi) of W_k[u]
+    std::vector<int> offsets;             // m_k: channel offset from the capture centre in channel steps (100 kHz | 10 kHz)
+    std::vector<int16_t> taps;            // [nch][plan->taps][2] (Wr, Wi) of W_k[u]
     std::vector<short2> phasor;           // [PERIOD]
-    int8_t *d_w;                          // [ngroups][8][128][64]
+    int8_t *d_w;                          // [ngroups][8 KPASS][128][64]
     int *d_rot;
     long long *d_corr;
     short2 *d_phasor;
@@ -401,7 +477,7 @@ struct nrsc5b_channelizer {
     PFN_cuTensorMapEncodeTiled_v12000 encode;
     // streaming (nrsc5b_chan_push / nrsc5b_chan_feed)
     long long pushed;                     // T: complex samples pushed since create / reset
-    uint8_t *d_stage;                     // [STAGE_CAP or STAGE_CAP_CS16]: carry (samples from 32 N(T) on) | the bytes being pushed
+    uint8_t *d_stage;                     // [stage_cap_cu8 or STAGE_CAP_CS16]: carry (samples from 32 N(T) on) | the bytes being pushed
     uint8_t *d_planes;                    // cs16: [2][PLANE_SAMPLES * 2] the x_hi and x_lo planes a launch reads
     CUtensorMap map_stage;                // what a streamed launch reads: d_stage (cu8) or d_planes (cs16)
     cudaEvent_t stage_done;               // the last work that used d_stage / d_planes (calls may come on different CUDA streams)
@@ -420,9 +496,25 @@ static double bessel_i0(double x)
     return s;
 }
 
-// The integer tables of the definition, on the host (no device needed): phasor[11907], taps[nch][256] = W_k[u] and, for
-// the kernel, the B operand bytes, the rotation steps and the per-channel offset corrections.
-static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor, std::vector<int16_t> &taps, std::vector<int8_t> *w,
+// The integer tables of the definition, on the host (no device needed): phasor[11907], taps[nch][plan taps] = W_k[u]
+// and, for the kernel, the B operand bytes, the rotation steps and the per-channel offset corrections.
+//
+// The bounds the kernel relies on, for either plan (S = sum_u |Wr| + |Wi| <= sqrt(2) 2^19 sum|h| + taps):
+//   tap bytes     |W| <= 2^19 max h, about 2^19 x 2 fc: 16 374 (FM), 16 197 (AM) < 127 x 256 + 127, so both bytes are int8;
+//   wgmma sums    a pass adds 512 products below 255 x 128: < 2^24, two passes < 2^25, far inside int32;
+//   cu8           |acc| <= 128 S < 2^28 (checked below): sum|h| = 1.40 (FM), 1.59 (AM, twice the taps but the same
+//                 relative cut-off, so only the window's longer tails add) bounds 128 S by 2^27.0 and 2^27.2; over
+//                 all offsets the tables reach 2^26.85 (FM, +-118) and 2^27.11 (AM, +-74);
+//   cs16          |A1| <= 128 S < 2^28 and |A2| <= 255 S < 2^29 by the same check, |acc| <= 2^15 S < 2^36.
+// So 512 taps hold at scale 2^19 and the AM plan keeps it.
+static bool offsets_ok(const Plan &pl, const int *offsets, int nch)
+{
+    for (int k = 0; pl.max_offset && k < nch; k++)
+        if (offsets[k] < -pl.max_offset || offsets[k] > pl.max_offset) return false;
+    return true;
+}
+
+static void make_tables(const Plan &pl, const int *offsets, int nch, std::vector<short2> &phasor, std::vector<int16_t> &taps, std::vector<int8_t> *w,
                         std::vector<int> *rot, std::vector<long long> *corr)
 {
     phasor.resize(PERIOD);
@@ -432,10 +524,11 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
     }
     for (int i = PERIOD / 2 + 1; i < PERIOD; i++)                          // exactly conjugate-symmetric: the kernel keeps half of it
         phasor[i] = make_short2(phasor[PERIOD - i].x, (short)-phasor[PERIOD - i].y);
-    // prototype low-pass: Kaiser-windowed sinc, -6 dB at 372 kHz: flat over a hybrid FM channel (+-200 kHz), >= 55 dB down from 544 kHz on (what folds onto the channel after /32), unit DC gain
+    // prototype low-pass: Kaiser-windowed sinc, unit DC gain
+    const int TAPS = pl.taps, KPASS = TAPS / PASS_TAPS;
     std::vector<double> h(TAPS);
     {
-        const double fc = 372000.0 / 23814000.0, beta = 5.65;
+        const double fc = pl.fc, beta = pl.beta;
         double sum = 0;
         for (int t = 0; t < TAPS; t++) {
             const double x = t - (TAPS - 1) / 2.0;
@@ -448,18 +541,18 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
     }
     const int ngroups = (nch + GROUP - 1) / GROUP;
     taps.assign((size_t)nch * TAPS * 2, 0);
-    if (w) w->assign((size_t)ngroups * W_BYTES, 0);
+    if (w) w->assign((size_t)ngroups * KPASS * W_BYTES, 0);
     if (rot) rot->assign(nch, 0);
     if (corr) corr->assign((size_t)nch * 2, 0);
     for (int k = 0; k < nch; k++) {
         const int m = offsets[k];
-        const long long step = (((long long)50 * m) % PERIOD + PERIOD) % PERIOD;
-        if (rot) (*rot)[k] = (int)((((long long)1600 * m) % PERIOD + PERIOD) % PERIOD);
+        const long long step = (((long long)pl.tap_step * m) % PERIOD + PERIOD) % PERIOD;
+        if (rot) (*rot)[k] = (int)((((long long)pl.mix_step * m) % PERIOD + PERIOD) % PERIOD);
         long long swr = 0, swi = 0, sabs = 0;
         const int g = k / GROUP, cl = k % GROUP;
         const int brow = 16 * (cl / 4) + 2 * (cl % 4);                   // B rows of the channel: brow + part (+ 8: low bytes)
         for (int u = 0; u < TAPS; u++) {
-            // W_k[u] = 2^19 h[255-u] e^{-j 2 pi 50 m u / 11907}, from the integer phasor table
+            // W_k[u] = 2^19 h[TAPS-1-u] e^{-j 2 pi tap_step m u / 11907}, from the integer phasor table
             const short2 ph = phasor[(size_t)((step * u) % PERIOD)];
             const double g0 = ldexp(h[TAPS - 1 - u], TAP_SCALE_LOG2) / 32767.0;
             const int wr = (int)lrint(g0 * ph.x), wi = (int)lrint(-g0 * ph.y);
@@ -477,7 +570,7 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
                     const int hi = (v + 128) >> 8, lo = v - 256 * hi;           // v = 256 hi + lo, both in [-128, 127]
                     if (hi < -128 || hi > 127) { fprintf(stderr, "nrsc5_b200: channeliser tap out of range\n"); abort(); }
                     const int kappa = 2 * u + comp, ck = kappa / CHUNK, b = kappa % CHUNK;
-                    const size_t base = ((size_t)(g * NCHUNK + ck) * TILE_N) * CHUNK;
+                    const size_t base = ((size_t)(g * KPASS * NCHUNK + ck) * TILE_N) * CHUNK;
                     (*w)[base + (size_t)(brow + part) * CHUNK + b] = (int8_t)hi;
                     (*w)[base + (size_t)(brow + 8 + part) * CHUNK + b] = (int8_t)lo;
                 }
@@ -491,21 +584,39 @@ static void make_tables(const int *offsets, int nch, std::vector<short2> &phasor
     }
 }
 
-/* The definition's tables without a device: taps[nch][256][2], phasor[11907][2] (either may be NULL). */
-extern "C" int nrsc5b_chan_make_tables(const int *offsets_100khz, int nch, int16_t *taps, int16_t *phasor)
+static int tables_of(const Plan &pl, const int *offsets, int nch, int16_t *taps, int16_t *phasor)
 {
-    if (!offsets_100khz || nch <= 0 || nch > 4096) return NRSC5B_EINVAL;
+    if (!offsets || nch <= 0 || nch > 4096 || !offsets_ok(pl, offsets, nch)) return NRSC5B_EINVAL;
     std::vector<short2> ph;
     std::vector<int16_t> tp;
-    make_tables(offsets_100khz, nch, ph, tp, nullptr, nullptr, nullptr);
+    make_tables(pl, offsets, nch, ph, tp, nullptr, nullptr, nullptr);
     if (taps) memcpy(taps, tp.data(), tp.size() * sizeof(int16_t));
     if (phasor) memcpy(phasor, ph.data(), PERIOD * sizeof(short2));
     return NRSC5B_OK;
 }
 
-static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16)
+/* The definition's tables without a device: taps[nch][256][2], phasor[11907][2] (either may be NULL). */
+extern "C" int nrsc5b_chan_make_tables(const int *offsets_100khz, int nch, int16_t *taps, int16_t *phasor)
 {
-    if (!out || !offsets_100khz || nch <= 0 || nch > 4096) return NRSC5B_EINVAL;
+    return tables_of(PLAN_FM, offsets_100khz, nch, taps, phasor);
+}
+
+/* The AM plan's: taps[nch][512][2], and the same phasor table. */
+extern "C" int nrsc5b_chan_make_tables_am(const int *offsets_10khz, int nch, int16_t *taps, int16_t *phasor)
+{
+    return tables_of(PLAN_AM, offsets_10khz, nch, taps, phasor);
+}
+
+using Kernel = void (*)(const CUtensorMap, const CUtensorMap, Params);
+static Kernel kernel_of(const nrsc5b_channelizer *c)
+{
+    if (c->plan->taps == PASS_TAPS) return c->cs16 ? k_channelize<true, 1> : k_channelize<false, 1>;
+    return c->cs16 ? k_channelize<true, 2> : k_channelize<false, 2>;
+}
+
+static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16)
+{
+    if (!out || !offsets_100khz || nch <= 0 || nch > 4096 || !offsets_ok(pl, offsets_100khz, nch)) return NRSC5B_EINVAL;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device >= ndev) {
         fprintf(stderr, "nrsc5_b200: no usable CUDA device (the channeliser has no CPU path)\n");
@@ -516,6 +627,7 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
     c->device = device;
     c->nch = nch;
     c->ngroups = (nch + GROUP - 1) / GROUP;
+    c->plan = &pl;
     c->cs16 = cs16;
     c->offsets.assign(offsets_100khz, offsets_100khz + nch);
     c->d_w = nullptr; c->d_rot = nullptr; c->d_corr = nullptr; c->d_phasor = nullptr;
@@ -532,7 +644,8 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
     std::vector<int8_t> w;
     std::vector<int> rot;
     std::vector<long long> corr;
-    make_tables(offsets_100khz, nch, c->phasor, c->taps, &w, &rot, &corr);
+    make_tables(pl, offsets_100khz, nch, c->phasor, c->taps, &w, &rot, &corr);
+    const int kpass = pl.taps / PASS_TAPS;
     bool ok = cudaMalloc(&c->d_w, w.size()) == cudaSuccess && cudaMalloc(&c->d_rot, nch * sizeof(int)) == cudaSuccess &&
               cudaMalloc(&c->d_corr, corr.size() * sizeof(long long)) == cudaSuccess &&
               cudaMalloc(&c->d_phasor, PERIOD * sizeof(short2)) == cudaSuccess;
@@ -541,8 +654,8 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
          cudaMemcpy(c->d_corr, corr.data(), corr.size() * sizeof(long long), cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(c->d_phasor, c->phasor.data(), PERIOD * sizeof(short2), cudaMemcpyHostToDevice) == cudaSuccess;
     if (ok) {
-        // taps as a [ngroups * 8 * 128 rows][64 B] matrix, boxes of 128 rows, 64-byte swizzle
-        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)c->ngroups * NCHUNK * TILE_N };
+        // taps as a [ngroups * 8 KPASS * 128 rows][64 B] matrix, boxes of 128 rows, 64-byte swizzle
+        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)c->ngroups * kpass * NCHUNK * TILE_N };
         const cuuint64_t strides[1] = { CHUNK };
         const cuuint32_t box[2] = { CHUNK, TILE_N }, es[2] = { 1, 1 };
         ok = c->encode(&c->map_w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_w, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -550,12 +663,12 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
     }
     // the streaming staging buffer (cu8) or the cs16 byte planes as a [rows][64 B] capture matrix (rows past a launch's
     // valid bytes only feed outputs the launch does not write)
-    const size_t stage_cap = cs16 ? STAGE_CAP_CS16 : STAGE_CAP, planes = cs16 ? 4 * PLANE_SAMPLES : 0;
+    const size_t stage_cap = cs16 ? STAGE_CAP_CS16 : stage_cap_cu8(pl.taps), planes = cs16 ? 4 * PLANE_SAMPLES : 0;
     ok = ok && cudaMalloc(&c->d_stage, stage_cap) == cudaSuccess && cudaMemset(c->d_stage, 0, stage_cap) == cudaSuccess &&
          cudaEventCreateWithFlags(&c->stage_done, cudaEventDisableTiming) == cudaSuccess;
     if (ok && cs16) ok = cudaMalloc(&c->d_planes, planes) == cudaSuccess && cudaMemset(c->d_planes, 0, planes) == cudaSuccess;
     if (ok) {
-        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)((cs16 ? planes : STAGE_CAP) / CHUNK) };
+        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)((cs16 ? planes : stage_cap) / CHUNK) };
         const cuuint64_t strides[1] = { CHUNK };
         const cuuint32_t box[2] = { CHUNK, TILE_M }, es[2] = { 1, 1 };
         ok = c->encode(&c->map_stage, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, cs16 ? c->d_planes : c->d_stage, dims, strides, box, es,
@@ -563,8 +676,7 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
     if (ok)
-        ok = cudaFuncSetAttribute(cs16 ? k_channelize<true> : k_channelize<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)SMEM_BYTES) == cudaSuccess;
+        ok = cudaFuncSetAttribute(kernel_of(c), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(kpass)) == cudaSuccess;
     if (!ok) {
         nrsc5b_chan_destroy(c);
         return NRSC5B_ECUDA;
@@ -575,12 +687,22 @@ static int create(nrsc5b_channelizer_t **out, int device, const int *offsets_100
 
 extern "C" int nrsc5b_chan_create(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch)
 {
-    return create(out, device, offsets_100khz, nch, false);
+    return create(PLAN_FM, out, device, offsets_100khz, nch, false);
 }
 
 extern "C" int nrsc5b_chan_create_cs16(nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch)
 {
-    return create(out, device, offsets_100khz, nch, true);
+    return create(PLAN_FM, out, device, offsets_100khz, nch, true);
+}
+
+extern "C" int nrsc5b_chan_create_am(nrsc5b_channelizer_t **out, int device, const int *offsets_10khz, int nch)
+{
+    return create(PLAN_AM, out, device, offsets_10khz, nch, false);
+}
+
+extern "C" int nrsc5b_chan_create_am_cs16(nrsc5b_channelizer_t **out, int device, const int *offsets_10khz, int nch)
+{
+    return create(PLAN_AM, out, device, offsets_10khz, nch, true);
 }
 
 extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
@@ -600,8 +722,8 @@ extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
     delete c;
 }
 
-/* The integer tables the definition is made of (for the numpy restatement in the tests): taps[nch][256][2] = (Wr, Wi)
- * of W_k[u], phasor[11907][2]. */
+/* The integer tables the definition is made of (for the numpy restatement in the tests): taps[nch][256 | 512][2] =
+ * (Wr, Wi) of W_k[u], phasor[11907][2]. */
 extern "C" int nrsc5b_chan_tables(nrsc5b_channelizer_t *c, int16_t *taps, int16_t *phasor)
 {
     if (!c) return NRSC5B_EINVAL;
@@ -610,11 +732,12 @@ extern "C" int nrsc5b_chan_tables(nrsc5b_channelizer_t *c, int16_t *taps, int16_
     return NRSC5B_OK;
 }
 
-// N(T): outputs whose 256-sample windows lie within the first T samples of a capture
-static long long outputs_of(long long samples) { return samples < TAPS ? 0 : (samples - TAPS) / DECIM + 1; }
+// N(T): outputs whose windows (one per 32 samples, as long as the plan's filter) lie within the first T samples of a capture
+static long long outputs_of(const Plan &pl, long long samples) { return samples < pl.taps ? 0 : (samples - pl.taps) / DECIM + 1; }
 
-/* How many output samples a capture of `nbytes` gives per channel: every output needs 256 input samples. */
-extern "C" long long nrsc5b_chan_outputs(size_t nbytes) { return outputs_of((long long)(nbytes / 2)); }
+/* How many output samples a capture of `nbytes` gives per channel: every output needs 256 input samples (AM: 512). */
+extern "C" long long nrsc5b_chan_outputs(size_t nbytes) { return outputs_of(PLAN_FM, (long long)(nbytes / 2)); }
+extern "C" long long nrsc5b_chan_outputs_am(size_t nbytes) { return outputs_of(PLAN_AM, (long long)(nbytes / 2)); }
 
 // outputs n0 .. n0 + nout - 1 of the capture whose sample 32 n0 is row 0 of map_x (cs16: of both planes in map_x):
 // output n0 + j of channel k goes to out + dst[k] + 2 j (dst null: k * out_stride)
@@ -638,10 +761,7 @@ static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0,
     long long slots = sms / c->ngroups;
     if (slots < 1) slots = 1;
     if (slots > p.tiles) slots = p.tiles;
-    if (c->cs16)
-        k_channelize<true><<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
-    else
-        k_channelize<false><<<(unsigned)(slots * c->ngroups), THREADS, SMEM_BYTES, stream>>>(map_x, c->map_w, p);
+    kernel_of(c)<<<(unsigned)(slots * c->ngroups), THREADS, smem_bytes(c->plan->taps / PASS_TAPS), stream>>>(map_x, c->map_w, p);
     return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
 }
 
@@ -664,7 +784,8 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
                      cudaStream_t stream)
 {
     if (!nsamples) return NRSC5B_OK;
-    const size_t bps = c->cs16 ? 4 : 2, cap = (c->cs16 ? STAGE_CAP_CS16 : STAGE_CAP) / bps;   // bytes per sample, samples staged
+    const Plan &pl = *c->plan;
+    const size_t bps = c->cs16 ? 4 : 2, cap = (c->cs16 ? STAGE_CAP_CS16 : stage_cap_cu8(pl.taps)) / bps;   // bytes per sample, samples staged
     // device memory: a device-to-device copy; page-locked host memory: DMA straight from it; pageable host memory: the
     // driver stages it (the copy returns once it has read the caller's bytes)
     cudaPointerAttributes attr;
@@ -675,19 +796,19 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
     if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;
     long long written = 0;
     for (size_t done = 0; done < nsamples;) {
-        const long long first = outputs_of(c->pushed);            // absolute index of staging row 0's output
+        const long long first = outputs_of(pl, c->pushed);        // absolute index of staging row 0's output
         const size_t carry = (size_t)(c->pushed - DECIM * first);
         const size_t piece = nsamples - done < cap - carry ? nsamples - done : cap - carry;
         if (cudaMemcpyAsync(c->d_stage + bps * carry, reinterpret_cast<const uint8_t *>(src) + bps * done, bps * piece, kind, stream) !=
             cudaSuccess)
             return NRSC5B_ECUDA;
-        const long long held = (long long)(carry + piece), nl = outputs_of(held);
+        const long long held = (long long)(carry + piece), nl = outputs_of(pl, held);
         if (nl > 0) {
             int rc = c->cs16 ? split_launch(c, reinterpret_cast<const int16_t *>(c->d_stage), held, first, nl, out + 2 * written, dst,
                                             out_stride, stream)
                              : launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream);
             if (rc) return rc;
-            k_move_carry<<<1, (unsigned)(128 * bps), 0, stream>>>(c->d_stage, bps * DECIM * nl, (int)(bps * (held - DECIM * nl)));
+            k_move_carry<<<1, (unsigned)(pl.taps * bps / 2), 0, stream>>>(c->d_stage, bps * DECIM * nl, (int)(bps * (held - DECIM * nl)));
             if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
         }
         c->pushed += (long long)piece;
@@ -707,7 +828,7 @@ extern "C" int nrsc5b_chan_reset(nrsc5b_channelizer_t *c)
 // nsamples complex samples of the handle's format at src (checked by the caller)
 static int push(nrsc5b_channelizer *c, const void *src, size_t nsamples, void *d_out, size_t out_stride, void *cuda_stream, long long *nout)
 {
-    const long long n = outputs_of(c->pushed + (long long)nsamples) - outputs_of(c->pushed);
+    const long long n = outputs_of(*c->plan, c->pushed + (long long)nsamples) - outputs_of(*c->plan, c->pushed);
     if (n > 0 && (!d_out || ((uintptr_t)d_out & 3) || (out_stride & 1) || (size_t)(2 * n) > out_stride)) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const int rc = stream_in(c, src, nsamples, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride,
@@ -735,7 +856,7 @@ extern "C" int nrsc5b_chan_push_cs16(nrsc5b_channelizer_t *c, const int16_t *cs1
 // nsamples complex samples of the handle's format at src (checked by the caller)
 static int feed(nrsc5b_channelizer *c, nrsc5b_engine_t *e, const int *streams, const void *src, size_t nsamples)
 {
-    const long long n = outputs_of(c->pushed + (long long)nsamples) - outputs_of(c->pushed);
+    const long long n = outputs_of(*c->plan, c->pushed + (long long)nsamples) - outputs_of(*c->plan, c->pushed);
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const size_t nch = (size_t)c->nch;
     if (!c->h_dst) {
@@ -758,7 +879,7 @@ static int feed(nrsc5b_channelizer *c, nrsc5b_engine_t *e, const int *streams, c
     if (cudaEventSynchronize(c->dst_copied[slot]) != cudaSuccess) return NRSC5B_ECUDA;
     long long *h_dst = c->h_dst + slot * nch, *d_dst = c->d_dst + slot * nch;
     FeedTarget t;
-    int rc = nbfeed_reserve(e, c->device, streams, c->nch, n, &t, h_dst);
+    int rc = nbfeed_reserve(e, c->device, c->plan->engine_mode, streams, c->nch, n, &t, h_dst);
     if (rc) return rc;
     if (n > 0) {
         if (cudaMemcpyAsync(d_dst, h_dst, nch * sizeof(long long), cudaMemcpyHostToDevice, t.stream) != cudaSuccess ||
@@ -790,7 +911,7 @@ extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8
 {
     if (!c || c->cs16 || !d_cu8 || !d_out || ((uintptr_t)d_cu8 & 63) || (nbytes & 63) || ((uintptr_t)d_out & 3) || (out_stride & 1))
         return NRSC5B_EINVAL;
-    const long long nout = nrsc5b_chan_outputs(nbytes);
+    const long long nout = outputs_of(*c->plan, (long long)(nbytes / 2));
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
@@ -812,7 +933,9 @@ extern "C" int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *
 {
     if (!c || !c->cs16 || !d_cs16 || !d_out || ((uintptr_t)d_cs16 & 15) || (nvalues & 1) || ((uintptr_t)d_out & 3) || (out_stride & 1))
         return NRSC5B_EINVAL;
-    const long long nout = nrsc5b_chan_outputs(nvalues);      // nvalues / 2 samples, as nbytes / 2 for cu8
+    const int TAPS = c->plan->taps;
+    const long long PIECE_OUT = piece_out(TAPS);
+    const long long nout = outputs_of(*c->plan, (long long)(nvalues / 2));
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
@@ -856,7 +979,7 @@ extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size
 {
     if (!c || c->cs16 || !cu8 || !out) return NRSC5B_EINVAL;
     nbytes &= ~(size_t)63;                                  // whole 64-byte rows (32 complex samples)
-    const long long nout = nrsc5b_chan_outputs(nbytes);
+    const long long nout = outputs_of(*c->plan, (long long)(nbytes / 2));
     if (nout <= 0) return NRSC5B_OK;
     return run_host(c, cu8, nbytes, nbytes, nout, out);
 }
@@ -864,7 +987,7 @@ extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size
 extern "C" int nrsc5b_chan_run_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, int16_t *out)
 {
     if (!c || !c->cs16 || !cs16 || !out || (nvalues & 1)) return NRSC5B_EINVAL;
-    const long long nout = nrsc5b_chan_outputs(nvalues);
+    const long long nout = outputs_of(*c->plan, (long long)(nvalues / 2));
     if (nout <= 0) return NRSC5B_OK;
     return run_host(c, cs16, 2 * nvalues, nvalues, nout, out);
 }

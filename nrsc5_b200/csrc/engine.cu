@@ -1467,10 +1467,10 @@ extern "C" int nrsc5b_attach_device_input(nrsc5b_engine_t *e, const void *dev_bu
 
 // The engine's side of nrsc5b_chan_feed (chan_feed.h): the channeliser writes cs16 samples straight behind each
 // target stream's data in the engine's own input buffers, on the engine's CUDA stream.
-int nbfeed_reserve(nrsc5b_engine_t *e, int device, const int *streams, int nch, long long nout, FeedTarget *t, long long *dst)
+int nbfeed_reserve(nrsc5b_engine_t *e, int device, int mode, const int *streams, int nch, long long nout, FeedTarget *t, long long *dst)
 {
     if (!e || !t || !dst || nch <= 0 || nout < 0) return NRSC5B_EINVAL;
-    if (e->cfg.mode != NRSC5B_MODE_FM || !e->dims.cs16 || !e->iq_owned || e->dp.iq != e->iq_owned || device != e->cfg.device ||
+    if (e->cfg.mode != mode || !e->dims.cs16 || !e->iq_owned || e->dp.iq != e->iq_owned || device != e->cfg.device ||
         e->in_flight)
         return NRSC5B_EINVAL;
     const int S = e->dims.nstreams;

@@ -320,3 +320,28 @@ def am_to_cu8(cs16: np.ndarray, gain: float = 1.0) -> np.ndarray:
     out[0::2] = up.real
     out[1::2] = up.imag
     return np.clip(np.rint(out + 127.0), 0, 255).astype(np.uint8)
+
+
+def make_am_band(stations, cs16: bool = True, noise_lsb: float = 3.0, seed: int = 9) -> np.ndarray:
+    """A band capture at 1 488 375 S/s for the wideband channeliser's AM plan (include/nrsc5_b200.h,
+    nrsc5b_chan_create_am): `stations` = (narrowband cs16 capture at 46 511.72 S/s, offset m in 10 kHz steps from the
+    capture centre, gain) each, interpolated by 32 as am_to_cu8 does, moved to its offset (10 kHz / 1 488 375 Hz =
+    80 / 11907 cycles per sample), scaled and summed over the length of the shortest one, with a noise floor of
+    `noise_lsb` LSB per component (channels without a station must not be exact zeros: see the header), and quantised.
+    Returns int16 I/Q interleaved (cs16=True; gain 1 keeps a station's cs16 level) or uint8 (cu8, where gain 1 / 64
+    keeps it at the channeliser's output)."""
+    from scipy.signal import resample_poly
+    n = min(c.size for c, _, _ in stations) // 2
+    t = np.arange(32 * n, dtype=np.float64)
+    wide = np.zeros(32 * n, dtype=np.complex128)
+    for c, m, gain in stations:
+        z = c[0:2 * n:2].astype(np.float64) + 1j * c[1:2 * n:2].astype(np.float64)
+        wide += resample_poly(z, 32, 1) * gain * np.exp(2j * np.pi * ((80 * m) % 11907) / 11907.0 * t)
+    rng = np.random.default_rng(seed)
+    wide += noise_lsb * (rng.standard_normal(wide.size) + 1j * rng.standard_normal(wide.size))
+    iq = np.empty(2 * wide.size)
+    iq[0::2] = wide.real
+    iq[1::2] = wide.imag
+    if cs16:
+        return np.clip(np.rint(iq), -32768, 32767).astype(np.int16)
+    return np.clip(np.rint(iq + 127.0), 0, 255).astype(np.uint8)
