@@ -238,6 +238,10 @@ int nrsc5b_halfband_fm(int device, const uint8_t *cu8, size_t npairs, int16_t *o
 int nrsc5b_viterbi_k7(int device, const int8_t *in, uint8_t *out, int len, int nframes);
 /* same; *fallbacks = frames the register-resident fast path handed to the exact fallback kernels */
 int nrsc5b_viterbi_k7_ex(int device, const int8_t *in, uint8_t *out, int len, int nframes, int *fallbacks);
+/* the register-resident fast path alone with chunks of ch steps (len, ch multiples of 32): dec[nframes][len+64][2] its
+ * decision words (bit 8*(n>>4) + (n&7) of word (n>>3)&1 set = new state n's survivor comes from the odd predecessor),
+ * retry[nframes] != 0 where it would hand the frame to the exact fallback */
+int nrsc5b_viterbi_k7_fast(int device, const int8_t *in, int len, int nframes, int ch, uint32_t *dec, int *retry);
 /* batch RS(255,247) decode in place; rc[n] = corrections or -1 (reference src/rs_decode.c:16) */
 int nrsc5b_rs_decode(int device, uint8_t *blocks255, int *rc, int nblocks);
 /* The AM chain's K=9 rate-1/3 tail-biting Viterbi decoder (reference src/conv_dec.c + src/conv_gen.h with K = 9 as

@@ -2239,6 +2239,46 @@ extern "C" int nrsc5b_viterbi_k7_ex(int device, const int8_t *in, uint8_t *out, 
     return viterbi_k7_impl(device, in, out, len, nframes, fallbacks);
 }
 
+/* The register-resident fast path alone, with chunks of `ch` steps: its decision words (every one of the len + 64
+ * steps) and its per-frame retry verdict - what the exact fallback would be asked to redo. */
+extern "C" int nrsc5b_viterbi_k7_fast(int device, const int8_t *in, int len, int nframes, int ch, uint32_t *dec, int *retry)
+{
+    int rc = use_device(device);
+    if (rc) return rc;
+    if (len < 32 || (len % 32) || nframes <= 0 || ch < 32 || (ch % 32)) return NRSC5B_EINVAL;
+    const int total = len + 64;
+    V64Args b;
+    b.stride = 1;
+    b.len = len;
+    b.ch = ch;
+    b.nch = (total + ch - 1) / ch;
+    b.dec_stride = (size_t)total;
+    int8_t *din = nullptr;
+    int *dflags = nullptr;                           // [ready | retry] x nframes
+    CK(cudaMalloc(&din, (size_t)nframes * 3 * len));
+    CK(cudaMemcpy(din, in, (size_t)nframes * 3 * len, cudaMemcpyHostToDevice));
+    std::vector<int> fl(2 * (size_t)nframes, 0);
+    for (int i = 0; i < nframes; i++) fl[i] = 1;
+    CK(cudaMalloc(&dflags, fl.size() * sizeof(int)));
+    CK(cudaMemcpy(dflags, fl.data(), fl.size() * sizeof(int), cudaMemcpyHostToDevice));
+    b.vin = din;
+    b.ready = dflags;
+    b.retry = dflags + nframes;
+    CK(cudaMalloc(&b.dec, (size_t)nframes * total * sizeof(uint2)));
+    CK(cudaMalloc(&b.bitsw, (size_t)nframes * (len / 32) * sizeof(uint32_t)));
+    CK(cudaMalloc(&b.vspec, (size_t)nframes * b.nch * 32 * sizeof(uint32_t)));
+    CK(cudaMalloc(&b.vend, (size_t)nframes * b.nch * 32 * sizeof(uint32_t)));
+    CK(cudaMalloc(&b.endstate, (size_t)nframes * sizeof(int)));
+    CK(cudaFuncSetAttribute(k_v64_emit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)V64_EMIT_SMEM));
+    launch_v64(b, nframes, 0);
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(dec, b.dec, (size_t)nframes * total * sizeof(uint2), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(retry, b.retry, (size_t)nframes * sizeof(int), cudaMemcpyDeviceToHost));
+    cudaFree(din); cudaFree(dflags); cudaFree(b.dec); cudaFree(b.bitsw);
+    cudaFree(b.vspec); cudaFree(b.vend); cudaFree(b.endstate);
+    return NRSC5B_OK;
+}
+
 static int viterbi_k7_impl(int device, const int8_t *in, uint8_t *out, int len, int nframes, int *fallbacks)
 {
     int rc = use_device(device);

@@ -97,6 +97,7 @@ def load_library():
     L.nrsc5b_halfband_fm.argtypes = [ci, vp, sz, vp]
     L.nrsc5b_viterbi_k7.argtypes = [ci, vp, vp, ci, ci]
     L.nrsc5b_viterbi_k7_ex.argtypes = [ci, vp, vp, ci, ci, ctypes.POINTER(ci)]
+    L.nrsc5b_viterbi_k7_fast.argtypes = [ci, vp, ci, ci, ci, vp, vp]
     L.nrsc5b_rs_decode.argtypes = [ci, vp, vp, ci]
     L.nrsc5b_fft2048.argtypes = [ci, vp, vp, ci]
     _lib = L
@@ -408,6 +409,19 @@ def viterbi_k7(soft: np.ndarray, length: int, device: int = 0, want_fallbacks: b
            "nrsc5b_viterbi_k7_ex")
     out = out.reshape(nframes, length)
     return (out, fb.value) if want_fallbacks else out
+
+
+def viterbi_k7_fast(soft: np.ndarray, length: int, chunk: int, device: int = 0):
+    """The K=7 decoder's register-resident fast path alone, with chunks of `chunk` steps: its decision words
+    [nframes][length + 64][2] (uint32) and its per-frame retry verdicts (True: it would hand the frame to the exact
+    fallback)."""
+    s = np.ascontiguousarray(soft, dtype=np.int8)
+    nframes = s.size // (3 * length)
+    dec = np.empty((nframes, length + 64, 2), dtype=np.uint32)
+    retry = np.empty(nframes, dtype=np.int32)
+    _check(load_library().nrsc5b_viterbi_k7_fast(device, s.ctypes.data, length, nframes, chunk, dec.ctypes.data,
+                                                 retry.ctypes.data), "nrsc5b_viterbi_k7_fast")
+    return dec, retry != 0
 
 
 def l2_frames(frames, device: int = 0, cap: int = 64 << 20):
