@@ -83,7 +83,6 @@ struct DemodSmem {
     // per team: the symbol's staged cu8 (IN_STRIDE bytes), then its NSYM decimated samples (short2); the FFT exchange
     // buffer aliases the start of both
     float2 buf[TEAMS][TEAM_SMEM / sizeof(float2)];
-    float2 symphase[TEAMS];
 };
 static_assert(FFT_SMEM_ELEMS * sizeof(float2) <= TEAM_SMEM && TEAM_SMEM % 16 == 0, "a team's FFT buffer");
 static_assert(DEMOD_RUN * FFT_THREADS >= NSYM && DEMOD_RUN % 2 == 1, "a symbol's runs");
@@ -142,9 +141,20 @@ struct SyncSmem {
     uint8_t *soft_w;                               // REC_SOFT_PM payload
     int do_search;
 };
+// A block's set-up: what its demod reads, and what a FINE block's prep commits to the stream's state.  k_stream<false>
+// computes it for the next block in front_sync (warp 1, beside the demap) and uses it if that block runs in FINE sync.
+struct BlockSet {
+    int samperr;                                   // window offset
+    int ok;                                        // set up by the last block's sync, not yet committed or discarded
+    float prev_angle, angle;                       // the NCO angle before and after the CFO correction
+    float theta;
+    float2 phase0, phase;                          // NCO phase at the block's first sample and after its 32 symbols
+};
 struct FrontSmem {
     float2 tw[FFT_TW];                             // FFT twiddle tables (fft.cuh)
     float2 nco[NSYM];                              // window[j] * exp(j*theta*j) of the current block
+    float2 symphase[BLK];                          // phase0 * exp(j*theta*NSYM*sym) of the current block's symbols
+    BlockSet blk;                                  // (k_stream<false>) the current block's set-up, or the next one's
     // reference carriers [symbol][reference slot], stored by the demodulating teams beside the kept bins (outside the
     // union: the sync phase reads them without a round trip through global memory), then rotated by the Costas loops.
     // The threads of a warp each walk one reference, symbol by symbol, so the slot index is the contiguous one.
@@ -275,15 +285,75 @@ __device__ __forceinline__ float2 acq_bandpass(const short2 *yy)
 }
 
 // NCO of a block in closed form, with the pulse shape folded in (acquire.c:243-252): nco[j] = shape[j] * exp(j*theta*j)
-__device__ __forceinline__ void fill_nco(const DevPtrs &p, float2 *nco, float theta, int t)
+__device__ __forceinline__ void fill_nco(const DevPtrs &p, float2 *nco, float theta, int t, int nthreads = FRONT_THREADS)
 {
-    for (int j = t; j < NSYM; j += FRONT_THREADS) {
+    for (int j = t; j < NSYM; j += nthreads) {
         float2 e = cexp_j(theta * (float)j);
         if (j < NCP || j >= NFFT) {
             const float w = __ldg(&p.shape[j]);
             e = make_float2(e.x * w, e.y * w);
         }
         nco[j] = e;
+    }
+}
+
+// phase of symbol `sym`'s kept bins (closed form of the NCO phase at the symbol's start): phase0 * exp(j*theta*NSYM*sym)
+__device__ __forceinline__ void fill_symphase(float2 *symphase, float theta, float2 phase0, int sym)
+{
+    double sn, cs;
+    sincos((double)theta * (double)(NSYM * sym), &sn, &cs);
+    symphase[sym] = cmul(phase0, make_float2((float)cs, (float)sn));
+}
+
+// A block's NCO from its window offset b.samperr and angle b.prev_angle (before the CFO correction) and the stream's
+// phase after the previous block (acquire.c:243-252)
+__device__ __forceinline__ void block_setup(BlockSet &b, const StreamState &st)
+{
+    const int adj = NSYM / 2 - b.samperr;
+    float angle = b.prev_angle;
+    angle = (float)((double)angle - 2 * M_PI * st.cfo);
+    const float pre = (float)(-adj) * angle / (float)NFFT;
+    const float2 ph = cmulf(st.phase, cexp_j(pre));
+    const float theta = angle / (float)NFFT;
+    // NCO phase after the 32 symbols of this block (acquire.c:250-252, closed form)
+    double sn, cs;
+    sincos((double)theta * (double)(NSYM * BLK), &sn, &cs);
+    const float2 pe = cmulf(ph, make_float2((float)cs, (float)sn));
+    const float nrm = sqrtf(pe.x * pe.x + pe.y * pe.y);
+    b.angle = angle;
+    b.theta = theta;
+    b.phase0 = ph;
+    b.phase = make_float2(pe.x / nrm, pe.y / nrm);
+}
+
+// sync_adjust (sync.c:769-777): the Costas phases of the kept bins follow the window's move by adj samples
+__device__ __forceinline__ void sync_adjust(const DevPtrs &p, int s, int adj, int t)
+{
+    if (adj == 0) return;
+    float *cp = p.cphase + (size_t)s * NFFT;
+    for (int i = t; i < SIDE; i += FRONT_THREADS) {
+        const int bl = LB0 + i, bu = UB1 - i;
+        cp[bl] = (float)((double)cp[bl] - (double)(adj * (bl - NFFT / 2) * 2) * M_PI / NFFT);
+        cp[bu] = (float)((double)cp[bu] - (double)(adj * (bu - NFFT / 2) * 2) * M_PI / NFFT);
+    }
+}
+
+// the block's parameters into the stream's state, and its REC_BLOCK record (thread 0)
+__device__ __forceinline__ void block_commit(const DevPtrs &p, const EngineDims &d, int s, const BlockSet &b, int state_in)
+{
+    StreamState &st = p.st[s];
+    st.phase0 = b.phase0;
+    st.theta = b.theta;
+    st.blk_samperr = b.samperr;
+    st.blk_state_in = state_in;
+    st.phase = b.phase;
+    uint8_t *w = log_reserve(p, d, s, REC_BLOCK, 32);
+    if (w) {
+        int *wi = reinterpret_cast<int *>(w);
+        float *wf = reinterpret_cast<float *>(w);
+        wi[0] = state_in; wi[1] = b.samperr; wf[2] = b.angle; wf[3] = b.phase0.x; wf[4] = b.phase0.y; wi[5] = st.cfo;
+        wi[6] = (int)(unsigned)(st.start & 0xffffffffLL);
+        wi[7] = (int)(st.start >> 32);
     }
 }
 
@@ -376,11 +446,10 @@ __device__ void front_acq_corr(const DevPtrs &p, int s, int t, int rank, int nra
 
 // prep, last part (owner CTA): timing and angle of the block - from the correlation sums when acquiring (mode 2) -,
 // sync_adjust, the block's NCO table and REC_BLOCK record
-__device__ void front_prep_finish(const DevPtrs &p, const EngineDims &d, int s, PrepSmem &sm, float2 *nco, int t, int mode)
+__device__ void front_prep_finish(const DevPtrs &p, const EngineDims &d, int s, PrepSmem &sm, float2 *nco, float2 *symphase,
+                                  BlockSet &b, int t, int mode)
 {
     StreamState &st = p.st[s];
-    __shared__ int sh_samperr;
-    __shared__ float sh_angle, sh_theta;
     const int state_in = st.state;
     if (mode == 2) {
         const float2 *gs = p.acq_sums + (size_t)s * NSYM;
@@ -425,95 +494,88 @@ __device__ void front_prep_finish(const DevPtrs &p, const EngineDims &d, int s, 
             const float factor = (st.prev_angle != 0.0f) ? 0.25f : 1.0f;
             const float angle = st.prev_angle + (angle_diff * factor);
             st.prev_angle = angle;
-            sh_angle = angle;
-            sh_samperr = (sm.red_idx[0] + NSYM - 15) % NSYM;
+            b.prev_angle = angle;
+            b.samperr = (sm.red_idx[0] + NSYM - 15) % NSYM;
             if (st.state == ST_NONE) st.state = ST_COARSE;
         }
     } else if (t == 0) {
-        sh_samperr = NSYM / 2 + st.samperr;
+        b.samperr = NSYM / 2 + st.samperr;
         st.samperr = 0;
         const float angle = st.prev_angle + (-st.angle);
         st.angle = 0;
         st.prev_angle = angle;
-        sh_angle = angle;
+        b.prev_angle = angle;
     }
     __syncthreads();
-
-    const int samperr = sh_samperr;
-    const int adj = NSYM / 2 - samperr;
-    if (adj != 0) {                                            // sync_adjust, sync.c:769-777
-        float *cp = p.cphase + (size_t)s * NFFT;
-        for (int i = t; i < SIDE; i += FRONT_THREADS) {
-            const int bl = LB0 + i, bu = UB1 - i;
-            cp[bl] = (float)((double)cp[bl] - (double)(adj * (bl - NFFT / 2) * 2) * M_PI / NFFT);
-            cp[bu] = (float)((double)cp[bu] - (double)(adj * (bu - NFFT / 2) * 2) * M_PI / NFFT);
-        }
-    }
+    sync_adjust(p, s, NSYM / 2 - b.samperr, t);
     if (t == 0) {
-        float angle = sh_angle;
-        angle = (float)((double)angle - 2 * M_PI * st.cfo);
-        const float pre = (float)(-adj) * angle / (float)NFFT;
-        const float2 ph = cmulf(st.phase, cexp_j(pre));
-        const float theta = angle / (float)NFFT;
-        st.phase0 = ph;
-        st.theta = theta;
-        sh_theta = theta;
-        st.blk_samperr = samperr;
-        st.blk_state_in = state_in;
-        // NCO phase after the 32 symbols of this block (acquire.c:250-252, closed form)
-        double sn, cs;
-        sincos((double)theta * (double)(NSYM * BLK), &sn, &cs);
-        const float2 pe = cmulf(ph, make_float2((float)cs, (float)sn));
-        const float nrm = sqrtf(pe.x * pe.x + pe.y * pe.y);
-        st.phase = make_float2(pe.x / nrm, pe.y / nrm);
-        uint8_t *w = log_reserve(p, d, s, REC_BLOCK, 32);
-        if (w) {
-            int *wi = reinterpret_cast<int *>(w);
-            float *wf = reinterpret_cast<float *>(w);
-            wi[0] = state_in; wi[1] = samperr; wf[2] = angle; wf[3] = ph.x; wf[4] = ph.y; wi[5] = st.cfo;
-            wi[6] = (int)(unsigned)(st.start & 0xffffffffLL);
-            wi[7] = (int)(st.start >> 32);
-        }
+        block_setup(b, st);
+        block_commit(p, d, s, b, state_in);
     }
     __syncthreads();
     // NCO of this block in closed form, with the pulse shape folded in (acquire.c:243-252):
     // nco[j] = shape[j] * exp(j*theta*j); the per-symbol phase is applied to the kept bins
-    fill_nco(p, nco, sh_theta, t);
+    fill_nco(p, nco, b.theta, t);
+    if (t >= FRONT_THREADS - BLK) fill_symphase(symphase, b.theta, b.phase0, t - (FRONT_THREADS - BLK));
     __syncthreads();
 }
 
 // prep of a block by ONE CTA (k_stream<false>, a stream per CTA): everything front_prep_begin / front_acq_tiles /
 // front_acq_corr / front_prep_finish do, in one piece - kept as one function because the 128-stream kernel is at its
-// 64-register ceiling and the split version costs it spills
-__device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, Acq1Smem &sm, float2 *nco, int t)
+// 64-register ceiling and the split version costs it spills.
+// A block in FINE sync whose set-up the previous block's front_sync computed (b.ok) only commits it: the state that
+// set-up was computed from has not changed since (in FINE sync only this prep and the sync's feedback write samperr,
+// angle, prev_angle, cfo and phase).  Its NCO table and symbol phases are filled by threads 1..1023 while thread 0
+// decides whether the block runs; a block that takes the other path fills them again below.
+__device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, Acq1Smem &sm, float2 *nco, float2 *symphase,
+                                  BlockSet &b, int t)
 {
     StreamState &st = p.st[s];
-    __shared__ int sh_active, sh_samperr;
-    __shared__ float sh_angle, sh_theta;
+    __shared__ int sh_active;
     if (t == 0) {
-        if (st.force_state >= 0) {
-            set_state(p, d, s, st.force_state);
-            st.force_state = -1;
-        }
-        // in_avail is advanced by asynchronous copies while this kernel runs
+        // the decision's loads first, all in flight together (the other threads wait for it); in_avail is advanced by
+        // asynchronous copies while this kernel runs
+        const int fs = st.force_state;
         const long long avail = *reinterpret_cast<volatile long long *>(&st.in_avail);
-        int act = avail >= 2 * (st.start + NACQ);
-        if (act && st.state == ST_FINE) {
+        const long long start = st.start;
+        const int psmi = st.psmi;
+        int state = st.state;
+        if (fs >= 0) {
+            set_state(p, d, s, fs);
+            st.force_state = -1;
+            state = fs;
+        }
+        int act = avail >= 2 * (start + NACQ);
+        if (act && state == ST_FINE) {
             // P3 / P4 frames (MP2, MP3, MP11) are decoded by kernel groups the host adds to the pass only when a
             // stream asks: wait at the block boundary until it has (nrsc5b_process looks at the flag).  Streams
             // in MP1 / MP5 / MP6 never pay for those launches.
-            const int need = px_need_of(c_compat_mode[st.psmi & 63]);
+            const int need = px_need_of(c_compat_mode[psmi & 63]);
             if (need & ~d.px_enabled) {
                 atomicOr(&p.ctl->px_need, (unsigned)need);
                 act = 0;
             }
         }
         st.active = act;
-        sh_active = act;
+        sh_active = act ? (state == ST_FINE && b.ok ? 2 : 1) : 0;
+        b.ok = 0;
         if (act) atomicAdd(&p.ctl->progress, 1ull);
+    } else {
+        fill_nco(p, nco, b.theta, t - 1, FRONT_THREADS - 1);
+        if (t >= FRONT_THREADS - BLK) fill_symphase(symphase, b.theta, b.phase0, t - (FRONT_THREADS - BLK));
     }
     __syncthreads();
     if (!sh_active) return false;
+    if (sh_active == 2) {
+        sync_adjust(p, s, NSYM / 2 - b.samperr, t);
+        if (t == 0) {
+            st.samperr = 0;
+            st.angle = 0;
+            st.prev_angle = b.prev_angle;
+            block_commit(p, d, s, b, ST_FINE);
+        }
+        return true;                                   // (k_stream reads the block's parameters from b)
+    }
 
     const uint8_t *iq = p.iq + (size_t)s * d.in_stride;
     const int state_in = st.state;
@@ -618,60 +680,29 @@ __device__ bool front_prep_single(const DevPtrs &p, const EngineDims &d, int s, 
             const float factor = (st.prev_angle != 0.0f) ? 0.25f : 1.0f;
             const float angle = st.prev_angle + (angle_diff * factor);
             st.prev_angle = angle;
-            sh_angle = angle;
-            sh_samperr = (sm.red_idx[0] + NSYM - 15) % NSYM;
+            b.prev_angle = angle;
+            b.samperr = (sm.red_idx[0] + NSYM - 15) % NSYM;
             if (st.state == ST_NONE) st.state = ST_COARSE;
         }
     } else if (t == 0) {
-        sh_samperr = NSYM / 2 + st.samperr;
+        b.samperr = NSYM / 2 + st.samperr;
         st.samperr = 0;
         const float angle = st.prev_angle + (-st.angle);
         st.angle = 0;
         st.prev_angle = angle;
-        sh_angle = angle;
+        b.prev_angle = angle;
     }
     __syncthreads();
-
-    const int samperr = sh_samperr;
-    const int adj = NSYM / 2 - samperr;
-    if (adj != 0) {                                            // sync_adjust, sync.c:769-777
-        float *cp = p.cphase + (size_t)s * NFFT;
-        for (int i = t; i < SIDE; i += FRONT_THREADS) {
-            const int bl = LB0 + i, bu = UB1 - i;
-            cp[bl] = (float)((double)cp[bl] - (double)(adj * (bl - NFFT / 2) * 2) * M_PI / NFFT);
-            cp[bu] = (float)((double)cp[bu] - (double)(adj * (bu - NFFT / 2) * 2) * M_PI / NFFT);
-        }
-    }
+    sync_adjust(p, s, NSYM / 2 - b.samperr, t);
     if (t == 0) {
-        float angle = sh_angle;
-        angle = (float)((double)angle - 2 * M_PI * st.cfo);
-        const float pre = (float)(-adj) * angle / (float)NFFT;
-        const float2 ph = cmulf(st.phase, cexp_j(pre));
-        const float theta = angle / (float)NFFT;
-        st.phase0 = ph;
-        st.theta = theta;
-        sh_theta = theta;
-        st.blk_samperr = samperr;
-        st.blk_state_in = state_in;
-        // NCO phase after the 32 symbols of this block (acquire.c:250-252, closed form)
-        double sn, cs;
-        sincos((double)theta * (double)(NSYM * BLK), &sn, &cs);
-        const float2 pe = cmulf(ph, make_float2((float)cs, (float)sn));
-        const float nrm = sqrtf(pe.x * pe.x + pe.y * pe.y);
-        st.phase = make_float2(pe.x / nrm, pe.y / nrm);
-        uint8_t *w = log_reserve(p, d, s, REC_BLOCK, 32);
-        if (w) {
-            int *wi = reinterpret_cast<int *>(w);
-            float *wf = reinterpret_cast<float *>(w);
-            wi[0] = state_in; wi[1] = samperr; wf[2] = angle; wf[3] = ph.x; wf[4] = ph.y; wi[5] = st.cfo;
-            wi[6] = (int)(unsigned)(st.start & 0xffffffffLL);
-            wi[7] = (int)(st.start >> 32);
-        }
+        block_setup(b, st);
+        block_commit(p, d, s, b, state_in);
     }
     __syncthreads();
     // NCO of this block in closed form, with the pulse shape folded in (acquire.c:243-252):
     // nco[j] = shape[j] * exp(j*theta*j); the per-symbol phase is applied to the kept bins
-    fill_nco(p, nco, sh_theta, t);
+    fill_nco(p, nco, b.theta, t);
+    if (t >= FRONT_THREADS - BLK) fill_symphase(symphase, b.theta, b.phase0, t - (FRONT_THREADS - BLK));
     __syncthreads();
     return true;
 }
@@ -686,8 +717,8 @@ __device__ __forceinline__ float2 sample_q15(short2 h)
 }
 
 __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sym, DemodSmem &sm, const float2 *nco,
-                            const float2 *tw, float2 (*zref)[ZS], const uint8_t *ref_plan,
-                            int half, int tl, long long start, int samperr, float theta, float2 phase0)
+                            const float2 *symphase, const float2 *tw, float2 (*zref)[ZS], const uint8_t *ref_plan,
+                            int half, int tl, long long start, int samperr)
 {
     float2 *buf = sm.buf[half];
     uint8_t *in = reinterpret_cast<uint8_t *>(buf);
@@ -725,11 +756,6 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
         asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
 #endif
     }
-    if (tl == 0) {
-        double sn, cs;
-        sincos((double)theta * (double)(NSYM * sym), &sn, &cs);
-        sm.symphase[half] = cmul(phase0, make_float2((float)cs, (float)sn));
-    }
     bar_sync(bar);
 
     // sw points at the 32-bit word holding input samples (2*base-14, 2*base-13): decimated sample j uses words j..j+7
@@ -762,7 +788,7 @@ __device__ void front_demod(const DevPtrs &p, const EngineDims &d, int s, int sy
     bar_sync(bar);                                        // every thread is done with the staged input and the samples
     float2 out[2][8];
     fft2048_block<true>(v, out, buf, tw, tl, bar);
-    const float2 sp = sm.symphase[half];                 // (rewritten behind the next symbol's first barrier)
+    const float2 sp = symphase[sym];
 
     // kept bins (sync.c:785-789, fftshift defines.h:123-138): with q = tl + 128 h and natural bin k = q + 256 k3,
     //   k3 = 5 (q >= 222) -> compact q - 222,  k3 = 6 (q <= 232) -> q + 34      (lower sideband, bins 478..744)
@@ -928,7 +954,7 @@ __device__ __forceinline__ int8_t soft_demap(float x, float mult)      // sync.c
 }
 
 template <bool CL>
-__device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSmem &sm, float2 (*zref)[ZS], int t)
+__device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSmem &sm, float2 (*zref)[ZS], BlockSet &b, int t)
 {
     StreamState &st = p.st[s];
     float *cfreq = p.cfreq + (size_t)s * NFFT;
@@ -1346,10 +1372,17 @@ __device__ void front_sync(const DevPtrs &p, const EngineDims &d, int s, SyncSme
                     angle += sm.cfq[MAXREF + i]; sum_xy += sm.fb_xy[1][i]; sum_x2 += x * x;
                 }
                 samperr = (float)((double)samperr - (double)((sum_xy / sum_x2) * (float)NFFT) * inv_2pi * BLK);
-                st.samperr = (int)roundf(samperr);
+                const int se = (int)roundf(samperr);
+                st.samperr = se;
                 angle /= (float)((ppb + 1) * 2);
                 st.angle = angle;
                 fb_angle = angle;
+                if (!CL) {                       // the next block's set-up, as its FINE prep would compute it
+                    b.samperr = NSYM / 2 + se;
+                    b.prev_angle = st.prev_angle + (-angle);
+                    block_setup(b, st);
+                    b.ok = 1;
+                }
             }
             fb_angle = __shfl_sync(0xffffffffu, fb_angle, 31);
             const int i = lane < MAXREF ? lane : lane - MAXREF;
@@ -1493,6 +1526,11 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         }
         sm.ref_plan[t] = (uint8_t)m;
     }
+    if (t == 0) {                                     // (the first block's prep fills its NCO tables from these)
+        sm.blk.ok = 0;
+        sm.blk.theta = 0.f;
+        sm.blk.phase0 = make_float2(0.f, 0.f);
+    }
     __syncthreads();
 
     const bool owner = !CL || rank == 0;
@@ -1516,12 +1554,12 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         // first - which the stream's CTAs share
         int mode = 0;
         if (!CL) {
-            if (nb < max_blocks && !st.p1_ready) mode = front_prep_single(p, d, s, sm.u.acq1, sm.nco, t) ? 1 : 0;
+            if (nb < max_blocks && !st.p1_ready) mode = front_prep_single(p, d, s, sm.u.acq1, sm.nco, sm.symphase, sm.blk, t) ? 1 : 0;
             if (mode == 0) break;
         } else {
             if (owner) {
                 if (nb < max_blocks && !st.p1_ready) mode = front_prep_begin(p, d, s, t);
-                if (mode == 1) front_prep_finish(p, d, s, sm.u.prep, sm.nco, t, 1);
+                if (mode == 1) front_prep_finish(p, d, s, sm.u.prep, sm.nco, sm.symphase, sm.blk, t, 1);
             }
             if (owner && t == 0) {
                 st.blk_go = mode;
@@ -1538,7 +1576,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
                 __threadfence();
                 cluster_barrier();
                 if (owner) {
-                    front_prep_finish(p, d, s, sm.u.prep, sm.nco, t, 2);
+                    front_prep_finish(p, d, s, sm.u.prep, sm.nco, sm.symphase, sm.blk, t, 2);
                     __threadfence();
                 }
                 cluster_barrier();                    // the block's parameters are in place
@@ -1546,16 +1584,18 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         }
         lap(st.blk_state_in == ST_FINE ? 2 : 1);
         const long long start = CL ? __ldcg(&st.start) : st.start;
-        const int samperr = CL ? __ldcg(&st.blk_samperr) : st.blk_samperr;
-        const float theta = CL ? __ldcg(&st.theta) : st.theta;
-        const float2 phase0 = CL ? __ldcg(&st.phase0) : st.phase0;
-        if (CL && !owner) {                                 // a helper CTA builds its own copy of the block's NCO table
+        // (k_stream<false>: thread 0 may still be committing the block's parameters to the stream's state)
+        const int samperr = CL ? __ldcg(&st.blk_samperr) : sm.blk.samperr;
+        if (CL && !owner) {                                 // a helper CTA builds its own copy of the block's NCO tables
+            const float theta = __ldcg(&st.theta);
             fill_nco(p, sm.nco, theta, t);
+            if (t >= FRONT_THREADS - BLK) fill_symphase(sm.symphase, theta, __ldcg(&st.phase0), t - (FRONT_THREADS - BLK));
             __syncthreads();
         }
 #pragma unroll 1
         for (int pass = 0; pass < BLK / (TEAMS * C); pass++)
-            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.tw, sm.zref, sm.ref_plan, team, tl, start, samperr, theta, phase0);
+            front_demod(p, d, s, (pass * C + rank) * TEAMS + team, sm.u.demod, sm.nco, sm.symphase, sm.tw, sm.zref, sm.ref_plan,
+                            team, tl, start, samperr);
         if (CL) {
             __threadfence();
             cluster_barrier();                        // every CTA's bins are in L2
@@ -1563,7 +1603,7 @@ __global__ void __launch_bounds__(FRONT_THREADS, 1) k_stream(DevPtrs p, EngineDi
         if (CL && !owner) continue;
         __syncthreads();
         lap(3);
-        front_sync<CL>(p, d, s, sm.u.sync, sm.zref, t);
+        front_sync<CL>(p, d, s, sm.u.sync, sm.zref, sm.blk, t);
         __syncthreads();
         lap(st.blk_state_in == ST_FINE ? 4 : 5);
     }
