@@ -371,6 +371,32 @@ int nrsc5b_chan_make_tables_am(const int *offsets_10khz, int nch, int16_t *taps,
  * nbytes % 64 == 0 */
 long long nrsc5b_chan_outputs_am(size_t nbytes);
 
+/* FM plans for narrower captures: one cu8 or cs16 capture at fs = D x 744 187.5 S/s, D = decim in {8, 16, 32}
+ * (5 953 500, 11 907 000 or 23 814 000 S/s) -> `nch` FM channels at 744 187.5 S/s cs16, the same output as the FM plan
+ * above.  Channel k is centred offsets_100khz[k] x 100 kHz from the capture's centre.  Integer-exact definition (m_k
+ * the offset, h_D the plan's 256-tap prototype, unit DC gain):
+ *     W_k[u] = round(2^14 D h_D[255-u] conj(P[((1600 / D) m_k u) mod 11907]) / 32767)         u < 256
+ *     cu8:   acc = sum_u W_k[u] (x[D n + u] - (127+127j));   v = (acc + 2^(s-1)) >> s,          s = 13 - log2(32 / D)
+ *     cs16:  acc = sum_u W_k[u]  x[D n + u];                 v = sat16((acc + 2^(t-1)) >> t),   t = 19 - log2(32 / D)
+ *     y[k][n] = sat16((v conj(P[(1600 m_k n) mod 11907]) + 2^14) >> 15)
+ *     N_D(T) = T >= 256 ? (T - 256) / D + 1 : 0;   carry = the samples from D N_D(T) on (at most 255)
+ * D = 32 is exactly the FM plan: nrsc5b_chan_create_fm(out, device, 32, ...) is nrsc5b_chan_create(out, device, ...).
+ * The tap scale 2^14 D keeps the largest tap near 16 380 for every D (the prototype's -6 dB point stays at 372 kHz, so
+ * its peak doubles each time D halves); the shifts keep the gain at 64 output LSB per cu8 LSB and 1 per cs16 LSB, and
+ * for x16 = 64 (x8 - 127) the cs16 output equals the cu8 output bit for bit.  h_D is a Kaiser-windowed sinc, -6 dB at
+ * 372 kHz, beta 9 for D = 16 and 8; its integer taps for channel 0 are within 0.001 dB over +-200 kHz and 85.4 dB
+ * (D = 16) and 80.2 dB (D = 8) down from 544 kHz on.  Offsets must lie inside the capture: |m_k| <= 59 for D = 16,
+ * <= 29 for D = 8; otherwise, and for a decim not in {8, 16, 32}: NRSC5B_EINVAL.  Every other entry point
+ * (nrsc5b_chan_run*, _push*, _feed*, _tables, _reset, _destroy) is shared and behaves as documented above with D in
+ * place of 32: nrsc5b_chan_feed* takes an FM cs16 engine. */
+int nrsc5b_chan_create_fm(nrsc5b_channelizer_t **out, int device, int decim, const int *offsets_100khz, int nch);
+int nrsc5b_chan_create_fm_cs16(nrsc5b_channelizer_t **out, int device, int decim, const int *offsets_100khz, int nch);
+/* the plan's tables without a device: taps[nch][256][2], phasor[11907][2]; either may be NULL */
+int nrsc5b_chan_make_tables_fm(int decim, const int *offsets_100khz, int nch, int16_t *taps, int16_t *phasor);
+/* output samples per channel of a capture of nbytes (cu8; cs16: int16 values) at D = decim: nbytes / 64 - 7 (D = 32),
+ * nbytes / 32 - 15 (D = 16), nbytes / 16 - 31 (D = 8) for nbytes % 64 == 0; NRSC5B_EINVAL for any other decim */
+long long nrsc5b_chan_outputs_fm(int decim, size_t nbytes);
+
 const char *nrsc5b_version(void);
 
 #ifdef __cplusplus

@@ -1,6 +1,7 @@
 """ctypes binding of the wideband channeliser (include/nrsc5_b200.h, csrc/channelizer.cu): one cu8 or cs16 capture at
-23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take; or, with
-band="am", one capture at 1 488 375 S/s -> AM channels (10 kHz grid) at 46 511.71875 S/s cs16 through a 512-tap bank.
+23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take; with
+decim=16 or 8, the same from a capture at 11 907 000 or 5 953 500 S/s (wide_rate(decim)); or, with band="am", one
+capture at 1 488 375 S/s -> AM channels (10 kHz grid) at 46 511.71875 S/s cs16 through a 512-tap bank.
 No CPU fallback: constructing a Channelizer without a CUDA device raises."""
 from __future__ import annotations
 
@@ -14,14 +15,26 @@ WIDE_RATE = 23814000.0          # 32 x 744 187.5
 AM_WIDE_RATE = 1488375.0        # 32 x 46 511.71875
 TAPS, PERIOD, DECIM = 256, 11907, 32
 TAPS_AM = 512
+FM_RATE = 744187.5              # every FM plan's output rate
+DECIMS = (8, 16, 32)            # the FM plans' decimations: captures at D x 744 187.5 S/s
 # band plan -> (taps per channel, suffix of the plan's own entry points)
 _BANDS = {"fm": (TAPS, ""), "am": (TAPS_AM, "_am")}
 
 
-def _band(band):
+def _band(band, decim=DECIM):
     if band not in _BANDS:
         raise ValueError(f"band: {band!r} is neither 'fm' nor 'am'")
+    if decim not in DECIMS:
+        raise ValueError(f"decim: {decim!r} is not one of {DECIMS}")
+    if band == "am" and decim != DECIM:
+        raise ValueError(f"decim: the AM plan decimates by {DECIM}, not {decim}")
     return _BANDS[band]
+
+
+def wide_rate(decim: int = DECIM) -> float:
+    """The capture rate of the FM plan that decimates by `decim`: decim x 744 187.5 S/s."""
+    _band("fm", decim)
+    return decim * FM_RATE
 
 
 def _lib():
@@ -50,53 +63,72 @@ def _lib():
         L.nrsc5b_chan_make_tables_am.argtypes = [vp, ci, vp, vp]
         L.nrsc5b_chan_outputs_am.argtypes = [sz]
         L.nrsc5b_chan_outputs_am.restype = ctypes.c_longlong
+        L.nrsc5b_chan_create_fm.argtypes = [ctypes.POINTER(vp), ci, ci, vp, ci]
+        L.nrsc5b_chan_create_fm_cs16.argtypes = [ctypes.POINTER(vp), ci, ci, vp, ci]
+        L.nrsc5b_chan_make_tables_fm.argtypes = [ci, vp, ci, vp, vp]
+        L.nrsc5b_chan_outputs_fm.argtypes = [ci, sz]
+        L.nrsc5b_chan_outputs_fm.restype = ctypes.c_longlong
         L._chan_ready = True
     return L
 
 
-def stream_outputs(pushed: int, nbytes: int, band: str = "fm") -> int:
+def stream_outputs(pushed: int, nbytes: int, band: str = "fm", decim: int = DECIM) -> int:
     """Outputs per channel a push of nbytes (cu8; cs16: int16 values) emits after `pushed` complex samples
-    (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // 32 + 1 for T >= 256, else 0 (band "am": 512 for 256)."""
-    ntaps = _band(band)[0]
+    (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // D + 1 for T >= 256, else 0, D = decim (band "am": 512
+    for 256)."""
+    ntaps = _band(band, decim)[0]
 
     def n(t):
-        return (t - ntaps) // DECIM + 1 if t >= ntaps else 0
+        return (t - ntaps) // decim + 1 if t >= ntaps else 0
     return n(pushed + nbytes // 2) - n(pushed)
 
 
-def make_tables(offsets_100khz, band: str = "fm"):
+def make_tables(offsets_100khz, band: str = "fm", decim: int = DECIM):
     """The integer tables of the definition, computed on the host (no device): taps[nch][256][2], phasor[11907][2]
-    (band "am": offsets in 10 kHz steps, taps[nch][512][2])."""
-    ntaps, sfx = _band(band)
+    (band "am": offsets in 10 kHz steps, taps[nch][512][2]; decim: the FM plan of a decim x 744 187.5 S/s capture)."""
+    ntaps, sfx = _band(band, decim)
     off = np.ascontiguousarray(offsets_100khz, dtype=np.int32)
     taps = np.empty((off.size, ntaps, 2), dtype=np.int16)
     ph = np.empty((PERIOD, 2), dtype=np.int16)
+    if decim != DECIM:
+        name = "nrsc5b_chan_make_tables_fm"
+        _check(_lib().nrsc5b_chan_make_tables_fm(decim, off.ctypes.data, off.size, taps.ctypes.data, ph.ctypes.data), name)
+        return taps, ph
     name = "nrsc5b_chan_make_tables" + sfx
     _check(getattr(_lib(), name)(off.ctypes.data, off.size, taps.ctypes.data, ph.ctypes.data), name)
     return taps, ph
 
 
-def outputs(nbytes: int, band: str = "fm") -> int:
+def outputs(nbytes: int, band: str = "fm", decim: int = DECIM) -> int:
     """Outputs per channel of a capture of nbytes cu8 bytes (or as many int16 values of cs16)."""
-    return int(getattr(_lib(), "nrsc5b_chan_outputs" + _band(band)[1])(nbytes & ~63))
+    sfx = _band(band, decim)[1]
+    if decim != DECIM:
+        return int(_lib().nrsc5b_chan_outputs_fm(decim, nbytes & ~63))
+    return int(getattr(_lib(), "nrsc5b_chan_outputs" + sfx)(nbytes & ~63))
 
 
 class Channelizer:
     """input_cs16=False: the capture is cu8 (uint8, lengths in bytes); True: cs16 (int16, lengths in int16 values,
     the _cs16 entry points).  Either way two input units make one complex sample.  band="am": the AM plan (offsets in
-    10 kHz steps of a 1 488 375 S/s capture, 512 taps); only create differs, every other call is the handle's."""
-    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False, band: str = "fm"):
+    10 kHz steps of a 1 488 375 S/s capture, 512 taps); decim=16 or 8: the FM plan of a capture at wide_rate(decim)
+    (offsets within +-59 or +-29).  Only create differs, every other call is the handle's."""
+    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False, band: str = "fm", decim: int = DECIM):
         self._L = _lib()
         self.band = band
-        self.taps = _band(band)[0]
+        self.decim = int(decim)
+        self.taps = _band(band, self.decim)[0]
         self.offsets = np.ascontiguousarray(offsets_100khz, dtype=np.int32)
         self.nch = int(self.offsets.size)
         self.input_cs16 = bool(input_cs16)
         self._dtype = np.int16 if self.input_cs16 else np.uint8
         self._sfx = "_cs16" if self.input_cs16 else ""
         self._h = ctypes.c_void_p()
-        name = "nrsc5b_chan_create" + _band(band)[1] + self._sfx
-        _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), name)
+        if self.decim != DECIM:
+            name = "nrsc5b_chan_create_fm" + self._sfx
+            _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.decim, self.offsets.ctypes.data, self.nch), name)
+        else:
+            name = "nrsc5b_chan_create" + _band(band)[1] + self._sfx
+            _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.offsets.ctypes.data, self.nch), name)
         self.device = device
         self.pushed = 0                 # T: complex samples pushed since create / reset (mirrors the handle's count)
 
@@ -131,7 +163,8 @@ class Channelizer:
         """Host capture (uint8, or int16 with input_cs16; I/Q interleaved) -> int16 array [nch][2 * outputs] (I, Q
         interleaved)."""
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
-        n = outputs(a.size, self.band)
+        # what the entry point writes: cu8 whole 64-byte rows, cs16 every complex sample
+        n = stream_outputs(0, a.size, self.band, self.decim) if self.input_cs16 else outputs(a.size, self.band, self.decim)
         out = np.empty((self.nch, 2 * max(n, 0)), dtype=np.int16)
         if n > 0:
             self._call("nrsc5b_chan_run", self._h, a.ctypes.data, a.size, out.ctypes.data)
@@ -162,7 +195,7 @@ class Channelizer:
         [nch][2 * n]: the outputs it completes.  Synchronous."""
         import torch
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
-        n = stream_outputs(self.pushed, a.size, self.band)
+        n = stream_outputs(self.pushed, a.size, self.band, self.decim)
         dev = torch.device("cuda", self.device)
         out = torch.empty((self.nch, 2 * max(n, 1)), dtype=torch.int16, device=dev)
         stream = torch.cuda.current_stream(dev)

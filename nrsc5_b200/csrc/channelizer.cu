@@ -68,6 +68,16 @@
 // one after the other + alignment, barriers and epilogue tables (25 744 B) = 222 352 B, the same total as the FM
 // instantiation's 64 KB of taps + four stages.  A consumer's loads and wgmmas therefore alternate; what overlaps is
 // the other consumer's loads, wgmmas and epilogue.  The input is 1/16 of the FM rate: residency, not speed, is the limit.
+//
+// FM plans at 11 907 000 and 5 953 500 S/s (nrsc5b_chan_create_fm*, D = 16 and 8; D = 32 is the FM plan above): the
+// same output rate, output mixer and epilogue, 256 taps at scale 2^14 D (the prototype's peak doubles each time D halves),
+//
+//     W_k[u] = round(2^14 D h_D[255-u] conj(P[((1600/D) m_k u) mod 11907]) / 32767)
+//     cu8:   v = (acc + 2^(s-1)) >> s,  s = 13 - log2(32/D);   cs16:  v = sat16((acc + 2^(t-1)) >> t),  t = 19 - log2(32/D)
+//     N_D(T) = T >= 256 ? (T - 256) / D + 1 : 0
+//
+// with the window of output n at x[D n ..].  In the kernel Q = 32 / D outputs share a capture-matrix row; Q tensor maps
+// over the same memory, 2 D bytes apart, feed the phase-major boxes of a tile (k_channelize's Q).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -109,12 +119,14 @@ static_assert(smem_bytes(1) <= 227 * 1024 && smem_bytes(2) <= 227 * 1024, "more 
 // cs16: the byte planes of up to PLANE_SAMPLES samples, x_hi rows first, then x_lo rows (one TMA map over both)
 constexpr long long PLANE_SAMPLES = (1ll << 22) + 256;
 constexpr int PLANE_ROWS = (int)(2 * PLANE_SAMPLES / CHUNK);
-// outputs per launch of the one-shot cs16 entry: 32 n + taps - 32 <= PLANE_SAMPLES (2^17 with 256 taps, 2^17 - 7 with 512)
-constexpr long long piece_out(int taps)
+// outputs per launch of the one-shot cs16 entry: D n + taps - D <= PLANE_SAMPLES (2^22 / D with 256 taps, 2^17 - 7 with
+// 512 taps at D = 32)
+constexpr long long piece_out(int taps, int decim)
 {
-    return (PLANE_SAMPLES - taps) / DECIM + 1 < (1ll << 17) ? (PLANE_SAMPLES - taps) / DECIM + 1 : 1ll << 17;
+    return (PLANE_SAMPLES - taps) / decim + 1 < (1ll << 22) / decim ? (PLANE_SAMPLES - taps) / decim + 1 : (1ll << 22) / decim;
 }
-static_assert(piece_out(256) == 1ll << 17 && DECIM * piece_out(512) + 512 - DECIM <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
+static_assert(piece_out(256, 32) == 1ll << 17 && DECIM * piece_out(512, 32) + 512 - DECIM <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
+static_assert(8 * piece_out(256, 8) + 256 - 8 <= PLANE_SAMPLES && 16 * piece_out(256, 16) + 256 - 16 <= PLANE_SAMPLES, "a one-shot piece must fit the planes");
 
 struct Params {
     int nch;                   // channels
@@ -232,14 +244,31 @@ __device__ __forceinline__ int ring_stage(unsigned it) { return KPASS == 1 ? it 
 template <int U, int KPASS>
 __device__ __forceinline__ unsigned ring_use(unsigned it) { return KPASS == 1 ? it / STAGES : (it / (2 * U)) * U + it % U; }
 
-// CS16: map_x addresses the two byte planes of a cs16 capture, the x_lo plane PLANE_ROWS rows after the x_hi plane.
+// The capture matrix as Q = 32 / D tensor maps over the same memory: map p starts at byte 2 D p (0 | 0, 32 | 0, 16,
+// 32, 48: all 16-byte aligned, as TMA requires), so output n = Q j + p reads rows j .. j + 7 of map p.
+template <int Q>
+struct XMaps {
+    CUtensorMap m[Q];
+};
+
+// CS16: the maps address the two byte planes of a cs16 capture, the x_lo plane PLANE_ROWS rows after the x_hi plane.
 // KPASS: K = 512 passes per output row (256 taps each).  Pass ps of output n reads capture-matrix rows n + 8 ps ..
 // n + 8 ps + 7 against tap chunks 8 ps .. 8 ps + 7 and adds into the same accumulators, so a 512-tap tile is two
 // stages of the ring per plane; with cs16 the x_hi plane is folded into A1 after all its passes, then the x_lo plane runs.
-template <bool CS16, int KPASS>
-__global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+// Q = 32 / D: consecutive outputs 2 D bytes apart, Q per capture-matrix row.  A tile is still 64 consecutive outputs;
+// its stage is filled phase-major, every K chunk as Q boxes of 64 / Q rows (a multiple of the 8-row swizzle atom),
+// box p holding outputs 64 tile + Q i + p, i < 64 / Q, from map p.  Tile row r is therefore output
+// 64 tile + Q (r mod 64 / Q) + r / (64 / Q).  The shifts follow the tap scale 2^14 D: s = 13 - log2 Q (cu8) and
+// t = 19 - log2 Q (cs16) keep unit DC gain.
+template <bool CS16, int KPASS, int Q>
+__global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant__ XMaps<Q> maps, const __grid_constant__ CUtensorMap map_w,
                                                            Params p)
 {
+    static_assert(Q == 1 || Q == 2 || Q == 4, "D = 32, 16 or 8");
+    static_assert(KPASS == 1 || Q == 1, "512-tap plans decimate by 32");
+    constexpr int LQ = Q == 1 ? 0 : (Q == 2 ? 1 : 2);
+    constexpr int SH_CU8 = SHIFT1 - LQ, SH_CS16 = TAP_SCALE_LOG2 - LQ;   // s, t
+    constexpr int BOX = TILE_M / Q;                                // rows per box, outputs per phase of a tile
     constexpr int PLANES = CS16 ? 2 : 1;                           // a tile takes PLANES * KPASS capture stages
     constexpr int NST = stages_of(KPASS), WB = KPASS * (int)W_BYTES, U = PLANES * KPASS;
     extern __shared__ uint8_t smem_raw[];
@@ -288,9 +317,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
                     const int s = ring_stage<U, KPASS>(it);
                     if (KPASS == 1 ? it >= STAGES : ring_use<U, KPASS>(it) > 0) mbar_wait(&bar.a_empty[s], (ring_use<U, KPASS>(it) - 1) & 1);
                     mbar_expect_tx(&bar.a_full[s], A_STAGE_BYTES);
-                    for (int c = 0; c < NCHUNK; c++)             // K chunk c of pass ps of output row n = capture-matrix row n + 8 ps + c
-                        tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK, &map_x, &bar.a_full[s], 0,
-                                    (int)(tile * TILE_M) + ps * NCHUNK + c + pl * PLANE_ROWS);
+                    for (int c = 0; c < NCHUNK; c++)             // K chunk c of pass ps of output row j = capture-matrix row j + 8 ps + c
+#pragma unroll
+                        for (int ph = 0; ph < Q; ph++)
+                            tma_load_2d(smem_a + (size_t)s * A_STAGE_BYTES + (size_t)c * TILE_M * CHUNK + (size_t)ph * BOX * CHUNK, &maps.m[ph],
+                                        &bar.a_full[s], 0, (int)(tile * BOX) + ps * NCHUNK + c + pl * PLANE_ROWS);
                 }
         }
         return;
@@ -362,7 +393,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
         // with the rotation step stays below 11907^2 < 2^32.
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            const long long n = tile * TILE_M + 16 * wwarp + (lane >> 2) + 8 * h;
+            const int r = 16 * wwarp + (lane >> 2) + 8 * h;       // tile row -> output: 64 tile + r when Q = 1
+            const long long n = Q == 1 ? tile * TILE_M + 16 * wwarp + (lane >> 2) + 8 * h : tile * TILE_M + (Q * (r % BOX) + r / BOX);
             const int nmod = (int)((p.n0mod + n) % PERIOD);
 #pragma unroll
             for (int i = 0; i < 8; i++) {
@@ -373,20 +405,21 @@ __global__ void __launch_bounds__(THREADS, 1) k_channelize(const __grid_constant
                 const int phx = v2.x, phy = up ? -v2.y : v2.y;
                 int vr, vi;
                 if constexpr (CS16) {
-                    // acc = 256 A1 + A2 < 2^36; with A1 = 2^11 (A1 >> 11) + (A1 & 2047):
-                    // (acc + 2^18) >> 19 = (A1 >> 11) + ((256 (A1 & 2047) + A2 + 2^18) >> 19), all terms below 2^30
+                    // acc = 256 A1 + A2 < 2^36; with A1 = 2^(t-8) (A1 >> (t-8)) + (A1 & (2^(t-8) - 1)), t = 19 (D = 32):
+                    // (acc + 2^(t-1)) >> t = (A1 >> (t-8)) + ((256 (A1 & (2^(t-8) - 1)) + A2 + 2^(t-1)) >> t), all terms below 2^30
+                    constexpr int SPLIT = SH_CS16 - 8;
                     const int a2r = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h]);           // |A2| < 2^29
                     const int a2i = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h]);
                     const int br = a1[4 * i + 2 * h], bi = a1[4 * i + 2 * h + 1];
-                    vr = (br >> 11) + ((((br & 2047) << 8) + a2r + (1 << 18)) >> 19);
-                    vi = (bi >> 11) + ((((bi & 2047) << 8) + a2i + (1 << 18)) >> 19);
+                    vr = (br >> SPLIT) + ((((br & ((1 << SPLIT) - 1)) << 8) + a2r + (1 << (SH_CS16 - 1))) >> SH_CS16);
+                    vi = (bi >> SPLIT) + ((((bi & ((1 << SPLIT) - 1)) << 8) + a2i + (1 << (SH_CS16 - 1))) >> SH_CS16);
                     vr = vr > 32767 ? 32767 : (vr < -32768 ? -32768 : vr);                            // sat16: the rotation stays in 32 bits
                     vi = vi > 32767 ? 32767 : (vi < -32768 ? -32768 : vi);
                 } else {
                     const int ar = (int)(256u * d[8 * i + 2 * h] + d[8 * i + 4 + 2 * h] - s_corr[2 * cl]);
                     const int ai = (int)(256u * d[8 * i + 2 * h + 1] + d[8 * i + 5 + 2 * h] - s_corr[2 * cl + 1]);
-                    vr = (ar + (1 << (SHIFT1 - 1))) >> SHIFT1;
-                    vi = (ai + (1 << (SHIFT1 - 1))) >> SHIFT1;
+                    vr = (ar + (1 << (SH_CU8 - 1))) >> SH_CU8;
+                    vi = (ai + (1 << (SH_CU8 - 1))) >> SH_CU8;
                 }
                 int zr = vr * phx + vi * phy, zi = vi * phx - vr * phy;        // v * conj(P)
                 zr = (zr + (1 << 14)) >> 15;
@@ -443,24 +476,37 @@ constexpr int DST_RING = 8;                                       // destination
 // ===========================================================================
 using namespace nbch;
 
-// A band plan: everything that differs between the FM grid (100 kHz channels of a 23 814 000 S/s capture) and the AM
-// grid (10 kHz channels of a 1 488 375 S/s capture).  Both decimate by 32 and share the 11907-entry phasor table:
-// 100 kHz / 23.814 MHz = 50 / 11907, 10 kHz / 1 488 375 Hz = 80 / 11907; the mixer steps are 32 x those.
+// A band plan: everything that differs between the FM grids (100 kHz channels of a D x 744 187.5 S/s capture, D = 32,
+// 16 or 8) and the AM grid (10 kHz channels of a 1 488 375 S/s capture).  All share the 11907-entry phasor table:
+// 100 kHz / (D x 744 187.5 Hz) = (1600 / D) / 11907, 10 kHz / 1 488 375 Hz = 80 / 11907; the mixer steps are D x those.
 struct Plan {
     int taps;                             // per channel: KPASS = taps / 256 passes of the kernel
+    int decim;                            // D: input samples per output; the tap scale is 2^14 D, the kernel's Q = 32 / D
     int tap_step, mix_step;               // phasor steps per input sample in W_k, per output sample in the mixer
     double fc, beta;                      // prototype: Kaiser-windowed sinc, -6 dB at fc (cycles per input sample)
     int max_offset;                       // |m_k| the capture holds (0: not limited)
     int engine_mode;                      // the engine nrsc5b_chan_feed may write into
 };
+static int log2_of(int v) { return v == 8 ? 3 : v == 16 ? 4 : 5; }   // D
+static int shift_cu8(const Plan &pl) { return SHIFT1 - (5 - log2_of(pl.decim)); }   // s: 13 at D = 32
 // FM: -6 dB at 372 kHz: flat over a hybrid FM channel (+-200 kHz), >= 55 dB down from 544 kHz on (what folds onto the
-// channel after /32)
-static const Plan PLAN_FM = { 256, 50, 1600, 372000.0 / 23814000.0, 5.65, 0, NRSC5B_MODE_FM };
+// channel after the decimation to 744 187.5 S/s)
+static const Plan PLAN_FM = { 256, 32, 50, 1600, 372000.0 / 23814000.0, 5.65, 0, NRSC5B_MODE_FM };
+// The same analogue spec at 11 907 000 and 5 953 500 S/s: the 256 taps span 2 and 4 times the time, so the transition
+// from 200 to 544 kHz is 2 and 4 times as many bins wide and a wider window (beta 9) fits in it.  Measured on the
+// integer taps of channel 0: D = 16 within 0.001 dB over +-200 kHz and 85.4 dB down from 544 kHz on, D = 8 within
+// 0.001 dB and 80.2 dB down (the rounding of taps at the 2^14 D scale is the floor there).  The captures span
+// +-5.95 and +-2.98 MHz: offsets beyond +-59 and +-29 are not in them.
+static const Plan PLAN_FM16 = { 256, 16, 100, 1600, 372000.0 / 11907000.0, 9.0, 59, NRSC5B_MODE_FM };
+static const Plan PLAN_FM8 = { 256, 8, 200, 1600, 372000.0 / 5953500.0, 9.0, 29, NRSC5B_MODE_FM };
 // AM: -6 dB at 23 kHz.  The integer taps of channel 0 are within +-0.001 dB up to 15 kHz (a hybrid AM channel) and
 // 87.1 dB down from 31.5 kHz on: what folds onto a channel after /32 are the stations k x 46.5 kHz away, which on the
 // 10 kHz grid land a few kHz off centre, on carriers 30 - 50 dB below an analog host.  The capture spans +-744 kHz:
 // offsets beyond +-74 are not in it.
-static const Plan PLAN_AM = { 512, 80, 2560, 23000.0 / 1488375.0, 8.8, 74, NRSC5B_MODE_AM };
+static const Plan PLAN_AM = { 512, 32, 80, 2560, 23000.0 / 1488375.0, 8.8, 74, NRSC5B_MODE_AM };
+
+// decim -> the FM plan (32: PLAN_FM itself); null for anything else
+static const Plan *fm_plan(int decim) { return decim == 32 ? &PLAN_FM : decim == 16 ? &PLAN_FM16 : decim == 8 ? &PLAN_FM8 : nullptr; }
 
 struct nrsc5b_channelizer {
     int device, nch, ngroups;
@@ -477,9 +523,9 @@ struct nrsc5b_channelizer {
     PFN_cuTensorMapEncodeTiled_v12000 encode;
     // streaming (nrsc5b_chan_push / nrsc5b_chan_feed)
     long long pushed;                     // T: complex samples pushed since create / reset
-    uint8_t *d_stage;                     // [stage_cap_cu8 or STAGE_CAP_CS16]: carry (samples from 32 N(T) on) | the bytes being pushed
+    uint8_t *d_stage;                     // [stage_cap_cu8 or STAGE_CAP_CS16]: carry (samples from D N(T) on) | the bytes being pushed
     uint8_t *d_planes;                    // cs16: [2][PLANE_SAMPLES * 2] the x_hi and x_lo planes a launch reads
-    CUtensorMap map_stage;                // what a streamed launch reads: d_stage (cu8) or d_planes (cs16)
+    CUtensorMap map_stage[4];             // what a streamed launch reads: d_stage (cu8) or d_planes (cs16), one map per phase
     cudaEvent_t stage_done;               // the last work that used d_stage / d_planes (calls may come on different CUDA streams)
     long long *h_dst, *d_dst;             // [DST_RING][nch] page-locked / device: per-channel destinations of a feed
     cudaEvent_t dst_copied[DST_RING];
@@ -499,12 +545,16 @@ static double bessel_i0(double x)
 // The integer tables of the definition, on the host (no device needed): phasor[11907], taps[nch][plan taps] = W_k[u]
 // and, for the kernel, the B operand bytes, the rotation steps and the per-channel offset corrections.
 //
-// The bounds the kernel relies on, for either plan (S = sum_u |Wr| + |Wi| <= sqrt(2) 2^19 sum|h| + taps):
-//   tap bytes     |W| <= 2^19 max h, about 2^19 x 2 fc: 16 374 (FM), 16 197 (AM) < 127 x 256 + 127, so both bytes are int8;
+// The bounds the kernel relies on, for every plan (S = sum_u |Wr| + |Wi| <= sqrt(2) 2^14 D sum|h| + taps):
+//   tap bytes     |W| <= 2^14 D max h, about 2^14 D x 2 fc: 16 374 (FM, every D), 16 197 (AM) < 127 x 256 + 127, so
+//                 both bytes are int8.  The -6 dB point stays at 372 kHz, so 2 fc doubles each time D halves; at a
+//                 fixed 2^19 the peak would be 32 760 (D = 16) and 65 520 (D = 8), hence the scale 2^14 D;
 //   wgmma sums    a pass adds 512 products below 255 x 128: < 2^24, two passes < 2^25, far inside int32;
-//   cu8           |acc| <= 128 S < 2^28 (checked below): sum|h| = 1.40 (FM), 1.59 (AM, twice the taps but the same
-//                 relative cut-off, so only the window's longer tails add) bounds 128 S by 2^27.0 and 2^27.2; over
-//                 all offsets the tables reach 2^26.85 (FM, +-118) and 2^27.11 (AM, +-74);
+//   cu8           |acc| <= 128 S < 2^(15 + s) <= 2^28 (checked below), so |v| < 2^15 after the shift by s = 13 - log2(32 / D)
+//                 and the rotation's products stay in 32 bits: sum|h| = 1.40 (FM D = 32), 1.59 (D = 16: beta 9), 1.88
+//                 (D = 8), 1.59 (AM, twice the taps but the same relative cut-off, so only the window's longer tails
+//                 add) bound 128 S / 2^s by 2^14.0, 2^14.2, 2^14.4 and 2^14.2; over all offsets the tables reach 2^26.85
+//                 (FM, +-118) and 2^27.11 (AM, +-74) at D = 32;
 //   cs16          |A1| <= 128 S < 2^28 and |A2| <= 255 S < 2^29 by the same check, |acc| <= 2^15 S < 2^36.
 // So 512 taps hold at scale 2^19 and the AM plan keeps it.
 static bool offsets_ok(const Plan &pl, const int *offsets, int nch)
@@ -526,6 +576,7 @@ static void make_tables(const Plan &pl, const int *offsets, int nch, std::vector
         phasor[i] = make_short2(phasor[PERIOD - i].x, (short)-phasor[PERIOD - i].y);
     // prototype low-pass: Kaiser-windowed sinc, unit DC gain
     const int TAPS = pl.taps, KPASS = TAPS / PASS_TAPS;
+    const int scale_log2 = TAP_SCALE_LOG2 - (5 - log2_of(pl.decim));   // 2^14 D
     std::vector<double> h(TAPS);
     {
         const double fc = pl.fc, beta = pl.beta;
@@ -552,9 +603,9 @@ static void make_tables(const Plan &pl, const int *offsets, int nch, std::vector
         const int g = k / GROUP, cl = k % GROUP;
         const int brow = 16 * (cl / 4) + 2 * (cl % 4);                   // B rows of the channel: brow + part (+ 8: low bytes)
         for (int u = 0; u < TAPS; u++) {
-            // W_k[u] = 2^19 h[TAPS-1-u] e^{-j 2 pi tap_step m u / 11907}, from the integer phasor table
+            // W_k[u] = 2^14 D h[TAPS-1-u] e^{-j 2 pi tap_step m u / 11907}, from the integer phasor table
             const short2 ph = phasor[(size_t)((step * u) % PERIOD)];
-            const double g0 = ldexp(h[TAPS - 1 - u], TAP_SCALE_LOG2) / 32767.0;
+            const double g0 = ldexp(h[TAPS - 1 - u], scale_log2) / 32767.0;
             const int wr = (int)lrint(g0 * ph.x), wi = (int)lrint(-g0 * ph.y);
             taps[((size_t)k * TAPS + u) * 2 + 0] = (int16_t)wr;
             taps[((size_t)k * TAPS + u) * 2 + 1] = (int16_t)wi;
@@ -575,8 +626,8 @@ static void make_tables(const Plan &pl, const int *offsets, int nch, std::vector
                     (*w)[base + (size_t)(brow + 8 + part) * CHUNK + b] = (int8_t)lo;
                 }
         }
-        // the kernel's epilogue computes in 32 bits (k_channelize): the filter output must stay below 2^28
-        if (128 * sabs >= (1ll << 28)) { fprintf(stderr, "nrsc5_b200: channeliser taps too large for the 32-bit epilogue\n"); abort(); }
+        // the kernel's epilogue computes in 32 bits (k_channelize): the filter output must stay below 2^(15 + s) <= 2^28
+        if (128 * sabs >= (1ll << (15 + shift_cu8(pl)))) { fprintf(stderr, "nrsc5_b200: channeliser taps too large for the 32-bit epilogue\n"); abort(); }
         if (corr) {
             (*corr)[2 * k + 0] = 127ll * (swr - swi);
             (*corr)[2 * k + 1] = 127ll * (swi + swr);
@@ -607,11 +658,42 @@ extern "C" int nrsc5b_chan_make_tables_am(const int *offsets_10khz, int nch, int
     return tables_of(PLAN_AM, offsets_10khz, nch, taps, phasor);
 }
 
-using Kernel = void (*)(const CUtensorMap, const CUtensorMap, Params);
-static Kernel kernel_of(const nrsc5b_channelizer *c)
+/* The FM plan at D x 744 187.5 S/s: taps[nch][256][2], the same phasor table. */
+extern "C" int nrsc5b_chan_make_tables_fm(int decim, const int *offsets_100khz, int nch, int16_t *taps, int16_t *phasor)
 {
-    if (c->plan->taps == PASS_TAPS) return c->cs16 ? k_channelize<true, 1> : k_channelize<false, 1>;
-    return c->cs16 ? k_channelize<true, 2> : k_channelize<false, 2>;
+    const Plan *pl = fm_plan(decim);
+    return pl ? tables_of(*pl, offsets_100khz, nch, taps, phasor) : NRSC5B_EINVAL;
+}
+
+// The kernel instantiation of a handle: 512 taps (AM) only at D = 32
+static const void *kernel_of(const nrsc5b_channelizer *c)
+{
+    const bool cs = c->cs16;
+    if (c->plan->taps != PASS_TAPS) return cs ? (const void *)k_channelize<true, 2, 1> : (const void *)k_channelize<false, 2, 1>;
+    switch (c->plan->decim) {
+    case 16: return cs ? (const void *)k_channelize<true, 1, 2> : (const void *)k_channelize<false, 1, 2>;
+    case 8: return cs ? (const void *)k_channelize<true, 1, 4> : (const void *)k_channelize<false, 1, 4>;
+    default: return cs ? (const void *)k_channelize<true, 1, 1> : (const void *)k_channelize<false, 1, 1>;
+    }
+}
+
+// Q = 32 / D maps of a capture matrix: map p over the nbytes bytes at base + 2 D p, [rows][64 B], boxes of 64 / Q rows,
+// 64-byte swizzle.  Rows past the end read as zero; only outputs the launch does not write touch them (an output's
+// window ends inside its map's whole rows).
+static bool encode_maps(nrsc5b_channelizer *c, CUtensorMap *maps, const void *base, size_t nbytes)
+{
+    const int D = c->plan->decim, Q = DECIM / D;
+    for (int ph = 0; ph < Q; ph++) {
+        const size_t off = (size_t)(2 * D * ph);
+        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)((nbytes - off) / CHUNK) };
+        const cuuint64_t strides[1] = { CHUNK };
+        const cuuint32_t box[2] = { CHUNK, (cuuint32_t)(TILE_M / Q) }, es[2] = { 1, 1 };
+        if (c->encode(&maps[ph], CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t *>(reinterpret_cast<const uint8_t *>(base) + off), dims,
+                      strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+            return false;
+    }
+    return true;
 }
 
 static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16)
@@ -667,14 +749,7 @@ static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const 
     ok = ok && cudaMalloc(&c->d_stage, stage_cap) == cudaSuccess && cudaMemset(c->d_stage, 0, stage_cap) == cudaSuccess &&
          cudaEventCreateWithFlags(&c->stage_done, cudaEventDisableTiming) == cudaSuccess;
     if (ok && cs16) ok = cudaMalloc(&c->d_planes, planes) == cudaSuccess && cudaMemset(c->d_planes, 0, planes) == cudaSuccess;
-    if (ok) {
-        const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)((cs16 ? planes : stage_cap) / CHUNK) };
-        const cuuint64_t strides[1] = { CHUNK };
-        const cuuint32_t box[2] = { CHUNK, TILE_M }, es[2] = { 1, 1 };
-        ok = c->encode(&c->map_stage, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, cs16 ? c->d_planes : c->d_stage, dims, strides, box, es,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-    }
+    if (ok) ok = encode_maps(c, c->map_stage, cs16 ? c->d_planes : c->d_stage, cs16 ? planes : stage_cap);
     if (ok)
         ok = cudaFuncSetAttribute(kernel_of(c), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(kpass)) == cudaSuccess;
     if (!ok) {
@@ -705,6 +780,19 @@ extern "C" int nrsc5b_chan_create_am_cs16(nrsc5b_channelizer_t **out, int device
     return create(PLAN_AM, out, device, offsets_10khz, nch, true);
 }
 
+// FM plans at D x 744 187.5 S/s, D = 32 (the plan of nrsc5b_chan_create itself), 16 or 8
+extern "C" int nrsc5b_chan_create_fm(nrsc5b_channelizer_t **out, int device, int decim, const int *offsets_100khz, int nch)
+{
+    const Plan *pl = fm_plan(decim);
+    return pl ? create(*pl, out, device, offsets_100khz, nch, false) : NRSC5B_EINVAL;
+}
+
+extern "C" int nrsc5b_chan_create_fm_cs16(nrsc5b_channelizer_t **out, int device, int decim, const int *offsets_100khz, int nch)
+{
+    const Plan *pl = fm_plan(decim);
+    return pl ? create(*pl, out, device, offsets_100khz, nch, true) : NRSC5B_EINVAL;
+}
+
 extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
 {
     if (!c) return;
@@ -732,16 +820,29 @@ extern "C" int nrsc5b_chan_tables(nrsc5b_channelizer_t *c, int16_t *taps, int16_
     return NRSC5B_OK;
 }
 
-// N(T): outputs whose windows (one per 32 samples, as long as the plan's filter) lie within the first T samples of a capture
-static long long outputs_of(const Plan &pl, long long samples) { return samples < pl.taps ? 0 : (samples - pl.taps) / DECIM + 1; }
+// N(T): outputs whose windows (one per D samples, as long as the plan's filter) lie within the first T samples of a capture
+static long long outputs_of(const Plan &pl, long long samples) { return samples < pl.taps ? 0 : (samples - pl.taps) / pl.decim + 1; }
 
 /* How many output samples a capture of `nbytes` gives per channel: every output needs 256 input samples (AM: 512). */
 extern "C" long long nrsc5b_chan_outputs(size_t nbytes) { return outputs_of(PLAN_FM, (long long)(nbytes / 2)); }
 extern "C" long long nrsc5b_chan_outputs_am(size_t nbytes) { return outputs_of(PLAN_AM, (long long)(nbytes / 2)); }
+extern "C" long long nrsc5b_chan_outputs_fm(int decim, size_t nbytes)
+{
+    const Plan *pl = fm_plan(decim);
+    return pl ? outputs_of(*pl, (long long)(nbytes / 2)) : NRSC5B_EINVAL;
+}
 
-// outputs n0 .. n0 + nout - 1 of the capture whose sample 32 n0 is row 0 of map_x (cs16: of both planes in map_x):
-// output n0 + j of channel k goes to out + dst[k] + 2 j (dst null: k * out_stride)
-static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0, long long nout, int16_t *out, const long long *dst,
+template <bool CS16, int KPASS, int Q>
+static void launch_k(const CUtensorMap *maps, const CUtensorMap &map_w, const Params &p, unsigned grid, cudaStream_t stream)
+{
+    XMaps<Q> m;
+    memcpy(m.m, maps, sizeof(m.m));
+    k_channelize<CS16, KPASS, Q><<<grid, THREADS, smem_bytes(KPASS), stream>>>(m, map_w, p);
+}
+
+// outputs n0 .. n0 + nout - 1 of the capture whose sample D n0 is row 0 of maps[0] (cs16: of both planes in the maps;
+// the plan's Q maps): output n0 + j of channel k goes to out + dst[k] + 2 j (dst null: k * out_stride)
+static int launch(nrsc5b_channelizer *c, const CUtensorMap *maps, long long n0, long long nout, int16_t *out, const long long *dst,
                   size_t out_stride, cudaStream_t stream)
 {
     Params p;
@@ -761,7 +862,12 @@ static int launch(nrsc5b_channelizer *c, const CUtensorMap &map_x, long long n0,
     long long slots = sms / c->ngroups;
     if (slots < 1) slots = 1;
     if (slots > p.tiles) slots = p.tiles;
-    kernel_of(c)<<<(unsigned)(slots * c->ngroups), THREADS, smem_bytes(c->plan->taps / PASS_TAPS), stream>>>(map_x, c->map_w, p);
+    const unsigned grid = (unsigned)(slots * c->ngroups);
+    const bool cs = c->cs16;
+    if (c->plan->taps != PASS_TAPS) (cs ? launch_k<true, 2, 1> : launch_k<false, 2, 1>)(maps, c->map_w, p, grid, stream);
+    else if (c->plan->decim == 16) (cs ? launch_k<true, 1, 2> : launch_k<false, 1, 2>)(maps, c->map_w, p, grid, stream);
+    else if (c->plan->decim == 8) (cs ? launch_k<true, 1, 4> : launch_k<false, 1, 4>)(maps, c->map_w, p, grid, stream);
+    else (cs ? launch_k<true, 1, 1> : launch_k<false, 1, 1>)(maps, c->map_w, p, grid, stream);
     return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
 }
 
@@ -786,6 +892,7 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
     if (!nsamples) return NRSC5B_OK;
     const Plan &pl = *c->plan;
     const size_t bps = c->cs16 ? 4 : 2, cap = (c->cs16 ? STAGE_CAP_CS16 : stage_cap_cu8(pl.taps)) / bps;   // bytes per sample, samples staged
+    const int D = pl.decim;
     // device memory: a device-to-device copy; page-locked host memory: DMA straight from it; pageable host memory: the
     // driver stages it (the copy returns once it has read the caller's bytes)
     cudaPointerAttributes attr;
@@ -797,7 +904,7 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
     long long written = 0;
     for (size_t done = 0; done < nsamples;) {
         const long long first = outputs_of(pl, c->pushed);        // absolute index of staging row 0's output
-        const size_t carry = (size_t)(c->pushed - DECIM * first);
+        const size_t carry = (size_t)(c->pushed - D * first);
         const size_t piece = nsamples - done < cap - carry ? nsamples - done : cap - carry;
         if (cudaMemcpyAsync(c->d_stage + bps * carry, reinterpret_cast<const uint8_t *>(src) + bps * done, bps * piece, kind, stream) !=
             cudaSuccess)
@@ -808,7 +915,7 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
                                             out_stride, stream)
                              : launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream);
             if (rc) return rc;
-            k_move_carry<<<1, (unsigned)(pl.taps * bps / 2), 0, stream>>>(c->d_stage, bps * DECIM * nl, (int)(bps * (held - DECIM * nl)));
+            k_move_carry<<<1, (unsigned)(pl.taps * bps / 2), 0, stream>>>(c->d_stage, bps * D * nl, (int)(bps * (held - D * nl)));
             if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
         }
         c->pushed += (long long)piece;
@@ -821,7 +928,7 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
 extern "C" int nrsc5b_chan_reset(nrsc5b_channelizer_t *c)
 {
     if (!c) return NRSC5B_EINVAL;
-    c->pushed = 0;                                            // the carry is what lies beyond 32 N(T): nothing now
+    c->pushed = 0;                                            // the carry is what lies beyond D N(T): nothing now
     return NRSC5B_OK;
 }
 
@@ -915,14 +1022,9 @@ extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
-    // the capture as a [rows][64 B] matrix; rows past the end read as zero (only rows of outputs >= nout touch them)
-    CUtensorMap map_x;
-    const cuuint64_t dims[2] = { CHUNK, (cuuint64_t)(nbytes / CHUNK) };
-    const cuuint64_t strides[1] = { CHUNK };
-    const cuuint32_t box[2] = { CHUNK, TILE_M }, es[2] = { 1, 1 };
-    if (c->encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void *>(d_cu8), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return NRSC5B_ECUDA;
+    // the capture as a [rows][64 B] matrix, one map per phase; rows past the end read as zero (only rows of outputs >= nout touch them)
+    CUtensorMap map_x[4];
+    if (!encode_maps(c, map_x, d_cu8, nbytes)) return NRSC5B_ECUDA;
     return launch(c, map_x, 0, nout, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -933,8 +1035,8 @@ extern "C" int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *
 {
     if (!c || !c->cs16 || !d_cs16 || !d_out || ((uintptr_t)d_cs16 & 15) || (nvalues & 1) || ((uintptr_t)d_out & 3) || (out_stride & 1))
         return NRSC5B_EINVAL;
-    const int TAPS = c->plan->taps;
-    const long long PIECE_OUT = piece_out(TAPS);
+    const int TAPS = c->plan->taps, D = c->plan->decim;
+    const long long PIECE_OUT = piece_out(TAPS, D);
     const long long nout = outputs_of(*c->plan, (long long)(nvalues / 2));
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
@@ -945,7 +1047,7 @@ extern "C" int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *
     if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;   // the planes are shared with the stream
     for (long long n0 = 0; n0 < nout; n0 += PIECE_OUT) {
         const long long nl = nout - n0 < PIECE_OUT ? nout - n0 : PIECE_OUT;
-        const int rc = split_launch(c, src + 2 * DECIM * n0, DECIM * nl + TAPS - DECIM, n0, nl, out + 2 * n0, nullptr, out_stride, stream);
+        const int rc = split_launch(c, src + 2 * D * n0, D * nl + TAPS - D, n0, nl, out + 2 * n0, nullptr, out_stride, stream);
         if (rc) return rc;
     }
     return cudaEventRecord(c->stage_done, stream) == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
