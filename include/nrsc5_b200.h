@@ -397,6 +397,47 @@ int nrsc5b_chan_make_tables_fm(int decim, const int *offsets_100khz, int nch, in
  * nbytes / 32 - 15 (D = 16), nbytes / 16 - 31 (D = 8) for nbytes % 64 == 0; NRSC5B_EINVAL for any other decim */
 long long nrsc5b_chan_outputs_fm(int decim, size_t nbytes);
 
+/* A capture at the radio's own rate: fs = rate_hz (integer Hz) -> the plan's capture rate R = D x 744 187.5 S/s (mode
+ * NRSC5B_MODE_FM, D = decim in {8, 16, 32}) or 1 488 375 S/s (NRSC5B_MODE_AM, decim = 32) through an exact polyphase
+ * resampler, then the plan's cs16 definition above, unchanged, on the result.  With R / fs = L / M in lowest terms:
+ *     b_n = floor(n M / L),  p_n = n M mod L
+ *     y[n] = sat16((sum_{j<64} G[p_n][j] x[b_n + j] + 2^13) >> 14)       (cu8 input: x = 64 (x8 - 127))
+ *     K(T) = T >= 64 ? ((T - 63) L - 1) / M + 1 : 0;   outputs of T input samples: N_plan(K(T))
+ * G[L][64] (nrsc5b_chan_resampler_tables): a Kaiser-windowed sinc (beta 8.41) designed at L fs, -6 dB at min(fs, R) / 2,
+ * split into L phases of 64 taps, each rounded to sum exactly 2^14 (unit DC gain) with sum |G[p]| < 2^16 (so the int32
+ * accumulation is exact).  The largest per-phase gain is about 2.8: full-scale cs16 input saturates y, as sat16 says.
+ * A cu8 handle equals a cs16 handle fed 64 (x8 - 127), bit for bit.
+ * Accepted: R / 32 <= fs <= 4 R and L <= 11 907 (every multiple of 2 kHz at D = 32, 1 kHz at D = 16, 500 Hz at D = 8,
+ * 125 Hz for AM).  The usable band is |f| <= f_p = (min(fs, R) - 11 fs / 128) / 2; a channel must lie inside it,
+ * |m| x 100 kHz + 200 kHz (FM) or |m| x 10 kHz + 15 kHz (AM) <= f_p, as well as inside the plan's own range.  Largest
+ * |offset| (nrsc5b_chan_resampler_tables), FM at every D it takes unless noted: 2.048 MS/s: 7; 2.4 MS/s: 8; 2.5 MS/s:
+ * 9; 3 MS/s: 11; 6 MS/s: 25; 8 MS/s: 24 (D = 8), 34; 10 MS/s: 23 (D = 8), 43; 20 MS/s: 19 (D = 8), 48 (D = 16),
+ * 89 (D = 32); 30.72 MS/s: 44 (D = 16), 103 (D = 32); 61.44 MS/s: 90 (D = 32).  AM: 768 kS/s: 33; 912 kS/s: 40;
+ * 2.4 MS/s: 62.
+ * Anything else: NRSC5B_EINVAL.  fs == R returns the plan's own handle (no stage), as nrsc5b_chan_create_fm does.
+ * Every other entry point (nrsc5b_chan_run*, _push*, _feed*, _tables, _reset, _destroy) is shared and keeps its rules,
+ * T counting input samples at fs; pushing a capture in pieces of any even size gives the one-shot output bit for bit.
+ * The one-shot entry points use every complex sample in both formats (no whole 64-byte rows), and one-shot device
+ * input needs 16-byte alignment only.  nrsc5b_chan_feed* takes the plan's engine (FM or AM, cs16, own buffers).
+ * Device scratch of a handle with a stage, whatever the capture size: 32 MiB + 2 KiB of staging and planes (as a cs16
+ * handle), 2 KiB for the streamed resampled carry (kept apart from the planes, so that a one-shot call between pushes
+ * leaves the stream as it was) and the table, L x 128 bytes (at most 1.5 MB). */
+int nrsc5b_chan_create_rate(nrsc5b_channelizer_t **out, int device, int mode, int decim, uint32_t rate_hz, const int *offsets, int nch);
+int nrsc5b_chan_create_rate_cs16(nrsc5b_channelizer_t **out, int device, int mode, int decim, uint32_t rate_hz, const int *offsets,
+                                 int nch);
+/* L, M, the largest usable |offset| and G[L][64] (may be NULL; any pointer may be NULL); no device needed.  fs == R:
+ * L = M = 1, the plan's own offset limit (0: none) and G the identity row. */
+int nrsc5b_chan_resampler_tables(int mode, int decim, uint32_t rate_hz, int *L, int *M, int *max_offset, int16_t *G);
+/* N_plan(K(T)) for T = samples input samples at fs; NRSC5B_EINVAL for a rate the library does not take */
+long long nrsc5b_chan_outputs_rate(int mode, int decim, uint32_t rate_hz, long long samples);
+/* The rate stage alone (kernel-level parity): host capture of nvalues cu8 bytes (cs16 = 0) or int16 values (cs16 = 1)
+ * -> host out[2 K(T)], y[0 .. K(T) - 1] I/Q interleaved; synchronous.  fs == R: NRSC5B_EINVAL (no stage). */
+int nrsc5b_resample(int device, int mode, int decim, uint32_t rate_hz, int cs16, const void *in, size_t nvalues, int16_t *out);
+/* The rate stage of a rate handle's one-shot device path alone (to time it apart from the channel bank): the k_resample
+ * launches nrsc5b_chan_run_device* makes for this capture (nvalues cu8 bytes or cs16 values, the handle's format,
+ * 16-byte aligned), into the handle's own scratch; no channel output.  NRSC5B_EINVAL on a handle without a stage. */
+int nrsc5b_chan_resample_device(nrsc5b_channelizer_t *c, const void *d_in, size_t nvalues, void *cuda_stream);
+
 const char *nrsc5b_version(void);
 
 #ifdef __cplusplus

@@ -1,7 +1,8 @@
 """ctypes binding of the wideband channeliser (include/nrsc5_b200.h, csrc/channelizer.cu): one cu8 or cs16 capture at
 23 814 000 S/s -> FM channels at 744 187.5 S/s cs16, the format nrsc5b_push_cs16 / input_push_cs16 take; with
 decim=16 or 8, the same from a capture at 11 907 000 or 5 953 500 S/s (wide_rate(decim)); or, with band="am", one
-capture at 1 488 375 S/s -> AM channels (10 kHz grid) at 46 511.71875 S/s cs16 through a 512-tap bank.
+capture at 1 488 375 S/s -> AM channels (10 kHz grid) at 46 511.71875 S/s cs16 through a 512-tap bank.  rate=fs: a
+capture at the radio's own rate (integer Hz) goes through an exact polyphase resampler to the chosen plan's rate first.
 No CPU fallback: constructing a Channelizer without a CUDA device raises."""
 from __future__ import annotations
 
@@ -19,6 +20,8 @@ FM_RATE = 744187.5              # every FM plan's output rate
 DECIMS = (8, 16, 32)            # the FM plans' decimations: captures at D x 744 187.5 S/s
 # band plan -> (taps per channel, suffix of the plan's own entry points)
 _BANDS = {"fm": (TAPS, ""), "am": (TAPS_AM, "_am")}
+_MODES = {"fm": 0, "am": 1}     # NRSC5B_MODE_FM, NRSC5B_MODE_AM
+RS_TAPS = 64                    # taps per phase of the rate stage
 
 
 def _band(band, decim=DECIM):
@@ -68,14 +71,77 @@ def _lib():
         L.nrsc5b_chan_make_tables_fm.argtypes = [ci, vp, ci, vp, vp]
         L.nrsc5b_chan_outputs_fm.argtypes = [ci, sz]
         L.nrsc5b_chan_outputs_fm.restype = ctypes.c_longlong
+        u32, ll = ctypes.c_uint32, ctypes.c_longlong
+        L.nrsc5b_chan_create_rate.argtypes = [ctypes.POINTER(vp), ci, ci, ci, u32, vp, ci]
+        L.nrsc5b_chan_create_rate_cs16.argtypes = [ctypes.POINTER(vp), ci, ci, ci, u32, vp, ci]
+        L.nrsc5b_chan_resampler_tables.argtypes = [ci, ci, u32, vp, vp, vp, vp]
+        L.nrsc5b_chan_outputs_rate.argtypes = [ci, ci, u32, ll]
+        L.nrsc5b_chan_outputs_rate.restype = ll
+        L.nrsc5b_resample.argtypes = [ci, ci, ci, u32, ci, vp, sz, vp]
+        L.nrsc5b_chan_resample_device.argtypes = [vp, vp, sz, vp]
         L._chan_ready = True
     return L
 
 
-def stream_outputs(pushed: int, nbytes: int, band: str = "fm", decim: int = DECIM) -> int:
+def _rate(rate, band, decim):
+    """rate (integer Hz) -> the mode / decim / rate the rate-stage entry points take; ValueError for a rate they refuse."""
+    _band(band, decim)
+    fs = int(rate)
+    if fs != rate or not 0 < fs < 1 << 32:
+        raise ValueError(f"rate: {rate!r} is not a positive integer number of Hz")
+    if _lib().nrsc5b_chan_outputs_rate(_MODES[band], decim, fs, 0) < 0:
+        raise ValueError(f"rate: {fs} Hz cannot be resampled to the {band} plan at decim={decim}")
+    return _MODES[band], decim, fs
+
+
+def _counts(rate, decim, band, G=None):
+    """(L, M, max_offset) of the rate stage; G: an int16 [L][64] array to receive its table as well."""
+    mode, decim, fs = _rate(rate, band, decim)
+    L, M, mo = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    _check(_lib().nrsc5b_chan_resampler_tables(mode, decim, fs, ctypes.byref(L), ctypes.byref(M), ctypes.byref(mo),
+                                               None if G is None else G.ctypes.data), "nrsc5b_chan_resampler_tables")
+    return L.value, M.value, mo.value
+
+
+def resampler_tables(rate, decim: int = DECIM, band: str = "fm"):
+    """The rate stage from a capture at `rate` Hz to the plan's rate, without a device: (L, M, max_offset, G) with
+    R / fs = L / M and G int16 [L][64] (fs == R: L = M = 1 and the identity row)."""
+    L = _counts(rate, decim, band)[0]
+    G = np.empty((L, RS_TAPS), dtype=np.int16)
+    L, M, mo = _counts(rate, decim, band, G)
+    return L, M, mo, G
+
+
+def resampled(samples: int, rate, decim: int = DECIM, band: str = "fm") -> int:
+    """K(T): resampled samples from T input samples at `rate`, by the header's formula (the library exports N_plan(K(T)),
+    nrsc5b_chan_outputs_rate, not K itself; this sizes resample()'s output, as stream_outputs sizes a push's)."""
+    L, M, _ = _counts(rate, decim, band)
+    if L == 1:
+        return samples
+    return ((samples - RS_TAPS + 1) * L - 1) // M + 1 if samples >= RS_TAPS else 0
+
+
+def resample(x: np.ndarray, rate, decim: int = DECIM, band: str = "fm", device: int = 0) -> np.ndarray:
+    """The rate stage alone on the device (nrsc5b_resample): a uint8 (cu8) or int16 (cs16) capture at `rate` -> int16
+    [2 K(T)], y I/Q interleaved."""
+    mode, decim, fs = _rate(rate, band, decim)
+    a = np.ascontiguousarray(x).reshape(-1)
+    assert a.dtype in (np.uint8, np.int16)
+    k = resampled(a.size // 2, rate, decim, band)
+    out = np.empty(2 * max(k, 1), dtype=np.int16)
+    _check(_lib().nrsc5b_resample(device, mode, decim, fs, int(a.dtype == np.int16), a.ctypes.data if a.size else None, a.size,
+                                  out.ctypes.data), "nrsc5b_resample")
+    return out[: 2 * k]
+
+
+def stream_outputs(pushed: int, nbytes: int, band: str = "fm", decim: int = DECIM, rate=None) -> int:
     """Outputs per channel a push of nbytes (cu8; cs16: int16 values) emits after `pushed` complex samples
     (include/nrsc5_b200.h): N(T') - N(T), N(T) = (T - 256) // D + 1 for T >= 256, else 0, D = decim (band "am": 512
-    for 256)."""
+    for 256); with rate, N_plan(K(T)) of a capture at `rate`."""
+    if rate is not None:
+        mode, decim, fs = _rate(rate, band, decim)
+        f = _lib().nrsc5b_chan_outputs_rate
+        return int(f(mode, decim, fs, pushed + nbytes // 2) - f(mode, decim, fs, pushed))
     ntaps = _band(band, decim)[0]
 
     def n(t):
@@ -99,8 +165,11 @@ def make_tables(offsets_100khz, band: str = "fm", decim: int = DECIM):
     return taps, ph
 
 
-def outputs(nbytes: int, band: str = "fm", decim: int = DECIM) -> int:
-    """Outputs per channel of a capture of nbytes cu8 bytes (or as many int16 values of cs16)."""
+def outputs(nbytes: int, band: str = "fm", decim: int = DECIM, rate=None) -> int:
+    """Outputs per channel of a capture of nbytes cu8 bytes (or as many int16 values of cs16); with rate, of a capture
+    at `rate` through the rate stage (every complex sample counts)."""
+    if rate is not None:
+        return stream_outputs(0, nbytes, band, decim, rate)
     sfx = _band(band, decim)[1]
     if decim != DECIM:
         return int(_lib().nrsc5b_chan_outputs_fm(decim, nbytes & ~63))
@@ -111,8 +180,11 @@ class Channelizer:
     """input_cs16=False: the capture is cu8 (uint8, lengths in bytes); True: cs16 (int16, lengths in int16 values,
     the _cs16 entry points).  Either way two input units make one complex sample.  band="am": the AM plan (offsets in
     10 kHz steps of a 1 488 375 S/s capture, 512 taps); decim=16 or 8: the FM plan of a capture at wide_rate(decim)
-    (offsets within +-59 or +-29).  Only create differs, every other call is the handle's."""
-    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False, band: str = "fm", decim: int = DECIM):
+    (offsets within +-59 or +-29); rate=fs: a capture at fs Hz, resampled to that plan's rate first (rate=None: the capture
+    is at the plan's rate; offsets within resampler_tables(rate, decim, band)[2]).  Only create differs, every other call
+    is the handle's."""
+    def __init__(self, offsets_100khz, device: int = 0, input_cs16: bool = False, band: str = "fm", decim: int = DECIM,
+                 rate=None):
         self._L = _lib()
         self.band = band
         self.decim = int(decim)
@@ -123,7 +195,13 @@ class Channelizer:
         self._dtype = np.int16 if self.input_cs16 else np.uint8
         self._sfx = "_cs16" if self.input_cs16 else ""
         self._h = ctypes.c_void_p()
-        if self.decim != DECIM:
+        # a capture at the plan's own rate is the plan itself (the library returns the plan's handle)
+        self.rate = None if rate is None or _counts(rate, self.decim, band)[0] == 1 else int(rate)
+        if rate is not None:
+            name = "nrsc5b_chan_create_rate" + self._sfx
+            mode, _, fs = _rate(rate, band, self.decim)
+            _check(getattr(self._L, name)(ctypes.byref(self._h), device, mode, self.decim, fs, self.offsets.ctypes.data, self.nch), name)
+        elif self.decim != DECIM:
             name = "nrsc5b_chan_create_fm" + self._sfx
             _check(getattr(self._L, name)(ctypes.byref(self._h), device, self.decim, self.offsets.ctypes.data, self.nch), name)
         else:
@@ -164,7 +242,10 @@ class Channelizer:
         interleaved)."""
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
         # what the entry point writes: cu8 whole 64-byte rows, cs16 every complex sample
-        n = stream_outputs(0, a.size, self.band, self.decim) if self.input_cs16 else outputs(a.size, self.band, self.decim)
+        if self.rate is not None:                  # every complex sample (an odd length is refused by the entry point)
+            n = stream_outputs(0, a.size, self.band, self.decim, self.rate)
+        else:
+            n = stream_outputs(0, a.size, self.band, self.decim) if self.input_cs16 else outputs(a.size, self.band, self.decim)
         out = np.empty((self.nch, 2 * max(n, 0)), dtype=np.int16)
         if n > 0:
             self._call("nrsc5b_chan_run", self._h, a.ctypes.data, a.size, out.ctypes.data)
@@ -174,6 +255,12 @@ class Channelizer:
         """Device capture (nbytes bytes of cu8, or nbytes int16 values of cs16) -> d_out[nch][out_stride]."""
         self._call("nrsc5b_chan_run_device", self._h, ctypes.c_void_p(d_cu8), nbytes, ctypes.c_void_p(d_out), out_stride,
                    ctypes.c_void_p(stream))
+
+    def resample_device(self, d_in: int, nvalues: int, stream: int = 0):
+        """The rate stage of run_device() alone (nrsc5b_chan_resample_device): the same k_resample launches into the
+        handle's scratch, no channel output; for timing the stage apart from the channel bank."""
+        _check(self._L.nrsc5b_chan_resample_device(self._h, ctypes.c_void_p(d_in), nvalues, ctypes.c_void_p(stream)),
+               "nrsc5b_chan_resample_device")
 
     # ---- streaming: a capture pushed in pieces; the outputs concatenate to run() of the whole capture ----
     def reset(self):
@@ -195,7 +282,7 @@ class Channelizer:
         [nch][2 * n]: the outputs it completes.  Synchronous."""
         import torch
         a = np.ascontiguousarray(cu8, dtype=self._dtype).reshape(-1)
-        n = stream_outputs(self.pushed, a.size, self.band, self.decim)
+        n = stream_outputs(self.pushed, a.size, self.band, self.decim, self.rate)
         dev = torch.device("cuda", self.device)
         out = torch.empty((self.nch, 2 * max(n, 1)), dtype=torch.int16, device=dev)
         stream = torch.cuda.current_stream(dev)

@@ -82,10 +82,12 @@
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <numeric>
 #include <vector>
 
 #include "../../include/nrsc5_b200.h"
@@ -465,6 +467,96 @@ __global__ void k_move_carry(uint8_t *buf, size_t from, int nbytes)
     if (i < nbytes) *reinterpret_cast<uint16_t *>(buf + i) = v;
 }
 
+// Rate stage (nrsc5b_chan_create_rate*): a capture at fs -> the plan's capture rate R, R / fs = L / M in lowest terms,
+//     y[n] = sat16((sum_{j<64} G[p_n][j] x[b_n + j] + 2^13) >> 14),   b_n = floor(n M / L),  p_n = n M mod L
+// (cu8: x = 64 (x8 - 127)), written straight into the byte planes the cs16 instantiations of k_channelize read.
+// A CTA takes RS_TILE consecutive outputs n0 + i: it stages their input span - at most (RS_TILE - 1) M / L + 65 samples,
+// M / L <= 4 (fs <= 4 R) - from the 16-byte boundary below it into shared memory with cp.async, then each thread reads
+// its phase row (64 taps, 128 B, L2-resident: L <= 11907 rows) and forms one output in exact int32 arithmetic
+// (sum_j |G[p][j]| < 2^16 is checked when the table is made, so |acc| + 2^13 < 2^31).
+constexpr int RS_TAPS = 64;                                       // J: taps per phase
+constexpr int RS_TILE = 256;                                      // outputs per CTA (one per thread)
+constexpr int RS_MAX_L = 11907;                                   // phases: the table stays within 1.5 MB
+constexpr int RS_CARRY = 512;                                     // resampled samples a streamed carry can hold (< the plan's taps)
+static_assert(RS_CARRY >= 2 * PASS_TAPS, "the carry holds fewer samples than the longest plan's taps");
+// staged samples: a span at M / L <= 4 and up to 7 below the 16-byte boundary, in whole 16-byte words of either format
+constexpr int RS_SPAN = ((RS_TILE - 1) * 4 + 1 + RS_TAPS + 7 + 7) / 8 * 8;
+
+__device__ __forceinline__ void cp_async16(void *dst, const void *src)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+
+// Outputs n = 0 .. nout - 1 of the stage, n at phase (p0 + n M) mod L and window start b0 + floor((p0 + n M) / L) of
+// the samples at `in` (16-byte aligned, in_len samples of 2 (cu8) or 4 (cs16) bytes; every window lies inside them);
+// output n goes to hi[2 n], hi[2 n + 1] (the signed high bytes of I, Q) and lo[...] (the low bytes).  The one 64-bit
+// product per CTA is its first output's q = p0 + n M, bounded by the launch, not by the capture.
+template <bool CU8>
+__global__ void __launch_bounds__(RS_TILE) k_resample(const uint8_t *__restrict__ in, long long in_len, long long b0, int p0, int L, int M,
+                                                      long long nout, const int16_t *__restrict__ G, uint8_t *__restrict__ hi,
+                                                      uint8_t *__restrict__ lo)
+{
+    constexpr int BPS = CU8 ? 2 : 4;                               // bytes per complex sample
+    __shared__ alignas(16) uint8_t raw[RS_SPAN * BPS];
+    __shared__ alignas(16) uint32_t conv[CU8 ? RS_SPAN : 1];       // cu8: the span as 16-bit (I, Q) = 64 (x8 - 127)
+    const long long nt0 = (long long)blockIdx.x * RS_TILE;
+    const int nt = (int)(nout - nt0 < RS_TILE ? nout - nt0 : RS_TILE);
+    const long long q0 = (long long)p0 + nt0 * M;
+    const long long bt = b0 + q0 / L;                              // the tile's first window start (absolute sample)
+    const int pt = (int)(q0 % L);
+    const int span = (int)(((long long)pt + (long long)(nt - 1) * M) / L) + RS_TAPS;   // samples the tile reads
+    const long long a0 = (bt * BPS) & ~15ll;                       // staging starts at the 16-byte boundary below bt
+    const int skip = (int)(bt * BPS - a0) / BPS;                   // samples before bt in the staging buffer
+    const int nbytes = (skip + span) * BPS;
+    const long long avail = in_len * BPS - a0;                     // bytes of the input from a0 on
+    for (int c = threadIdx.x; 16 * c < nbytes; c += RS_TILE) {
+        if (16ll * c + 16 <= avail)
+            cp_async16(raw + 16 * c, in + a0 + 16 * c);
+        else
+            for (int k = 0; k < 16; k++) raw[16 * c + k] = 16ll * c + k < avail ? in[a0 + 16 * c + k] : 0;
+    }
+    asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+    __syncthreads();
+    const uint32_t *xs;
+    if constexpr (CU8) {
+        for (int s = threadIdx.x; s < skip + span; s += RS_TILE) {
+            const uint32_t v = *reinterpret_cast<const uint16_t *>(raw + 2 * s);
+            const int xr = 64 * ((int)(v & 255) - 127), xi = 64 * ((int)(v >> 8) - 127);
+            conv[s] = (uint32_t)(uint16_t)(int16_t)xr | ((uint32_t)(uint16_t)(int16_t)xi << 16);
+        }
+        __syncthreads();
+        xs = conv + skip;
+    } else {
+        xs = reinterpret_cast<const uint32_t *>(raw) + skip;
+    }
+    const int i = threadIdx.x;
+    if (i >= nt) return;
+    const int qi = pt + i * M;                                     // < 11907 + 255 x 47628 < 2^24
+    const int b = qi / L, p = qi - b * L;
+    const uint4 *row = reinterpret_cast<const uint4 *>(G + (size_t)p * RS_TAPS);
+    const uint32_t *x = xs + b;
+    int ar = 0, ai = 0;
+#pragma unroll
+    for (int c = 0; c < RS_TAPS / 8; c++) {
+        const uint4 w = __ldg(row + c);
+        const uint32_t ws[4] = { w.x, w.y, w.z, w.w };
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int g0 = (int)(ws[k] << 16) >> 16, g1 = (int)ws[k] >> 16;
+            const uint32_t x0 = x[8 * c + 2 * k], x1 = x[8 * c + 2 * k + 1];
+            ar += g0 * ((int)(x0 << 16) >> 16) + g1 * ((int)(x1 << 16) >> 16);
+            ai += g0 * ((int)x0 >> 16) + g1 * ((int)x1 >> 16);
+        }
+    }
+    int yr = (ar + (1 << 13)) >> 14, yi = (ai + (1 << 13)) >> 14;
+    yr = yr > 32767 ? 32767 : (yr < -32768 ? -32768 : yr);
+    yi = yi > 32767 ? 32767 : (yi < -32768 ? -32768 : yi);
+    const uint32_t packed = (uint32_t)(uint16_t)(int16_t)yr | ((uint32_t)(uint16_t)(int16_t)yi << 16);
+    const long long n = nt0 + i;
+    reinterpret_cast<uint16_t *>(hi)[n] = (uint16_t)__byte_perm(packed, 0, 0x0031);   // high bytes of I, Q
+    reinterpret_cast<uint16_t *>(lo)[n] = (uint16_t)__byte_perm(packed, 0, 0x0020);   // low bytes
+}
+
 constexpr size_t stage_cap_cu8(int taps) { return (4u << 20) + 2 * (size_t)taps; }   // cu8 staging: the carry (< 2 taps bytes) + 4 MiB of new capture
 constexpr size_t STAGE_CAP_CS16 = 4 * PLANE_SAMPLES;              // cs16 staging: as many samples as the planes hold (16 MiB + 1 KiB)
 constexpr int DST_RING = 8;                                       // destination tables in flight (nrsc5b_chan_feed)
@@ -530,7 +622,18 @@ struct nrsc5b_channelizer {
     long long *h_dst, *d_dst;             // [DST_RING][nch] page-locked / device: per-channel destinations of a feed
     cudaEvent_t dst_copied[DST_RING];
     unsigned dst_pos;
+    // rate stage (nrsc5b_chan_create_rate*; rs_L = 0: none): the capture at fs goes through k_resample into d_planes,
+    // and the plan runs its cs16 definition on the result.  d_stage then holds the raw input from b_{K(T)} on.
+    int rs_L, rs_M;                       // R / fs = L / M
+    int16_t *d_G;                         // [rs_L][64] the phase table
+    uint8_t *d_rcarry;                    // [2 planes][2 RS_CARRY] the streamed resampled carry (the planes are shared)
+    long long rs_k;                       // K(T): resampled samples made since create / reset
+    long long rs_b;                       // b_{K(T)}: the input sample at row 0 of d_stage
+    int rs_p;                             // p_{K(T)} = K(T) M mod L
 };
+
+// the kernel reads the byte planes of a cs16 capture (a cs16 handle, or any handle with a rate stage)
+static bool reads_planes(const nrsc5b_channelizer *c) { return c->cs16 || c->rs_L; }
 
 static double bessel_i0(double x)
 {
@@ -665,10 +768,149 @@ extern "C" int nrsc5b_chan_make_tables_fm(int decim, const int *offsets_100khz, 
     return pl ? tables_of(*pl, offsets_100khz, nch, taps, phasor) : NRSC5B_EINVAL;
 }
 
+// ---- rate stage: a capture at any integer rate fs -> the plan's capture rate R through a polyphase resampler ----
+//
+// R / fs = L / M in lowest terms (2R and 2 fs are integers).  G[L][64]: a Kaiser-windowed sinc (beta 8.41, 85 dB) of
+// 64 L taps designed at L fs, -6 dB at min(fs, R) / 2, phase p holding taps p + (63 - j) L, j < 64.  Each phase is
+// scaled to sum 2^14 and rounded by largest remainder, so that it sums to exactly 2^14 (DC gain exactly 1).  The usable
+// band is |f| <= f_p = (min(fs, R) - 11 fs / 128) / 2 (11 fs / 128: the Kaiser transition width of 85 dB over 64 taps
+// per phase, 5.37 fs / 64, rounded up), in integers 512 f_p = 128 min(2 fs, 2 R) - 22 fs; a channel must lie inside
+// it: |m| step + half width <= f_p (FM: 100 kHz steps, 200 kHz; AM: 10 kHz, 15 kHz).
+constexpr double RS_BETA = 8.41;
+struct RateStage {
+    const Plan *plan;
+    int L, M;                             // R / fs = L / M
+    int max_offset;                       // largest usable |m| (fs == R: the plan's own limit, 0 = none)
+    uint32_t rate;                        // fs
+};
+
+// 2R: twice the plan's capture rate, an integer for every plan (D x 1 488 375 for FM, 2 976 750 for AM)
+static long long twice_rate(const Plan &pl) { return pl.engine_mode == NRSC5B_MODE_AM ? 2976750ll : (long long)pl.decim * 1488375ll; }
+
+// mode / decim / fs -> the stage's counts; false for anything the library does not take
+static bool rate_stage(int mode, int decim, uint32_t rate_hz, RateStage *rs)
+{
+    const Plan *pl = mode == NRSC5B_MODE_FM ? fm_plan(decim) : mode == NRSC5B_MODE_AM && decim == DECIM ? &PLAN_AM : nullptr;
+    if (!pl || rate_hz == 0) return false;
+    const long long r2 = twice_rate(*pl), f2 = 2ll * rate_hz;
+    if (64ll * rate_hz < r2 || f2 > 4 * r2) return false;          // R / 32 <= fs <= 4 R
+    const long long g = std::gcd(r2, f2);
+    if (r2 / g > RS_MAX_L) return false;
+    rs->plan = pl;
+    rs->L = (int)(r2 / g);
+    rs->M = (int)(f2 / g);
+    rs->rate = rate_hz;
+    if (rs->L == 1 && rs->M == 1) {                                // fs == R: the plan itself
+        rs->max_offset = pl->max_offset;
+        return true;
+    }
+    const bool am = pl->engine_mode == NRSC5B_MODE_AM;
+    const long long step = am ? 10000 : 100000, half = am ? 15000 : 200000;
+    const long long fp512 = 128 * std::min(f2, r2) - 22ll * rate_hz;
+    if (fp512 < 512 * half) return false;                          // not even channel 0 fits
+    long long mo = (fp512 - 512 * half) / (512 * step);
+    if (pl->max_offset && mo > pl->max_offset) mo = pl->max_offset;
+    rs->max_offset = (int)mo;
+    return true;
+}
+
+static bool rate_offsets_ok(const RateStage &rs, const int *offsets, int nch)
+{
+    if (rs.L == 1) return offsets_ok(*rs.plan, offsets, nch);
+    for (int k = 0; k < nch; k++)
+        if (offsets[k] < -rs.max_offset || offsets[k] > rs.max_offset) return false;
+    return true;
+}
+
+// K(T): resampled samples whose 64-sample windows lie within the first T input samples
+static long long resampled_of(int L, int M, long long samples) { return samples < RS_TAPS ? 0 : ((samples - RS_TAPS + 1) * L - 1) / M + 1; }
+
+// G[L][64] of a stage (L > 1).  Checks that every tap fits int16 and every phase's sum |G| < 2^16, which keeps the
+// kernel's int32 accumulation exact for any cs16 input: |acc| + 2^13 <= 2^15 (2^16 - 1) + 2^13 < 2^31.
+static void design_resampler(const RateStage &rs, std::vector<int16_t> &G)
+{
+    const int L = rs.L, N = RS_TAPS * L;
+    const double fc = std::min(2.0 * rs.rate, (double)twice_rate(*rs.plan)) / 4.0 / ((double)L * rs.rate);   // cycles per sample at L fs
+    const double i0b = bessel_i0(RS_BETA);
+    std::vector<double> h(N);
+    for (int t = 0; t < N; t++) {
+        const double x = t - (N - 1) / 2.0;
+        const double sinc = fabs(x) < 1e-12 ? 2 * fc : sin(2 * M_PI * fc * x) / (M_PI * x);
+        const double r = 2.0 * t / (N - 1) - 1.0;
+        h[t] = sinc * bessel_i0(RS_BETA * sqrt(std::max(0.0, 1 - r * r))) / i0b;
+    }
+    G.assign((size_t)L * RS_TAPS, 0);
+    for (int p = 0; p < L; p++) {
+        double v[RS_TAPS], sum = 0;
+        for (int j = 0; j < RS_TAPS; j++) sum += (v[j] = h[p + (size_t)(RS_TAPS - 1 - j) * L]);
+        long long fl[RS_TAPS], total = 0;
+        int order[RS_TAPS];
+        for (int j = 0; j < RS_TAPS; j++) {
+            v[j] *= 16384.0 / sum;
+            fl[j] = (long long)floor(v[j]);
+            total += fl[j];
+            order[j] = j;
+        }
+        // the 2^14 - sum(floor) units go to the taps with the largest remainders (ties: the lower j)
+        std::stable_sort(order, order + RS_TAPS, [&](int a, int b) { return v[a] - fl[a] > v[b] - fl[b]; });
+        const long long extra = 16384 - total;
+        long long sabs = 0;
+        for (int j = 0; j < RS_TAPS; j++) {
+            const long long g = fl[order[j]] + (j < extra ? 1 : 0);
+            if (g < -32768 || g > 32767) { fprintf(stderr, "nrsc5_b200: resampler tap out of range\n"); abort(); }
+            G[(size_t)p * RS_TAPS + order[j]] = (int16_t)g;
+            sabs += g < 0 ? -g : g;
+        }
+        if (extra < 0 || extra > RS_TAPS || sabs >= 65536) { fprintf(stderr, "nrsc5_b200: resampler phase out of bounds\n"); abort(); }
+    }
+}
+
+// nout resampled samples into the planes from sample `at` on: phase p0 and window start b0 (input samples counted from
+// `in`, 16-byte aligned, in_len samples of 2 (cu8) or 4 (cs16) bytes)
+static int launch_resample(bool cu8, const void *in, long long in_len, long long b0, int p0, int L, int M, long long nout, const int16_t *d_G,
+                           uint8_t *planes, long long at, cudaStream_t stream)
+{
+    if (nout <= 0) return NRSC5B_OK;
+    const unsigned grid = (unsigned)((nout + RS_TILE - 1) / RS_TILE);
+    const uint8_t *src = reinterpret_cast<const uint8_t *>(in);
+    uint8_t *hi = planes + 2 * at, *lo = planes + 2 * PLANE_SAMPLES + 2 * at;
+    if (cu8) k_resample<true><<<grid, RS_TILE, 0, stream>>>(src, in_len, b0, p0, L, M, nout, d_G, hi, lo);
+    else k_resample<false><<<grid, RS_TILE, 0, stream>>>(src, in_len, b0, p0, L, M, nout, d_G, hi, lo);
+    return cudaGetLastError() == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+}
+
+static bool attach_rate(nrsc5b_channelizer *c, const RateStage &rs)
+{
+    std::vector<int16_t> G;
+    design_resampler(rs, G);
+    c->rs_L = rs.L;
+    c->rs_M = rs.M;
+    return cudaMalloc(&c->d_rcarry, 4 * RS_CARRY) == cudaSuccess && cudaMalloc(&c->d_G, G.size() * sizeof(int16_t)) == cudaSuccess &&
+           cudaMemcpy(c->d_G, G.data(), G.size() * sizeof(int16_t), cudaMemcpyHostToDevice) == cudaSuccess;
+}
+
+/* L, M, the largest usable |offset| and G[L][64] of a rate stage, without a device (fs == R: L = M = 1 and G the
+ * identity row). */
+extern "C" int nrsc5b_chan_resampler_tables(int mode, int decim, uint32_t rate_hz, int *L, int *M, int *max_offset, int16_t *G)
+{
+    RateStage rs;
+    if (!rate_stage(mode, decim, rate_hz, &rs)) return NRSC5B_EINVAL;
+    if (L) *L = rs.L;
+    if (M) *M = rs.M;
+    if (max_offset) *max_offset = rs.max_offset;
+    if (G) {
+        std::vector<int16_t> g;
+        if (rs.L == 1) g.assign(RS_TAPS, 0), g[0] = 16384;
+        else design_resampler(rs, g);
+        memcpy(G, g.data(), g.size() * sizeof(int16_t));
+    }
+    return NRSC5B_OK;
+}
+
 // The kernel instantiation of a handle: 512 taps (AM) only at D = 32
 static const void *kernel_of(const nrsc5b_channelizer *c)
 {
-    const bool cs = c->cs16;
+    const bool cs = reads_planes(c);
     if (c->plan->taps != PASS_TAPS) return cs ? (const void *)k_channelize<true, 2, 1> : (const void *)k_channelize<false, 2, 1>;
     switch (c->plan->decim) {
     case 16: return cs ? (const void *)k_channelize<true, 1, 2> : (const void *)k_channelize<false, 1, 2>;
@@ -696,7 +938,8 @@ static bool encode_maps(nrsc5b_channelizer *c, CUtensorMap *maps, const void *ba
     return true;
 }
 
-static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16)
+static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const int *offsets_100khz, int nch, bool cs16,
+                  const RateStage *rs = nullptr)
 {
     if (!out || !offsets_100khz || nch <= 0 || nch > 4096 || !offsets_ok(pl, offsets_100khz, nch)) return NRSC5B_EINVAL;
     int ndev = 0;
@@ -716,6 +959,7 @@ static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const 
     c->pushed = 0; c->d_stage = nullptr; c->d_planes = nullptr; c->stage_done = nullptr;
     c->h_dst = nullptr; c->d_dst = nullptr; c->dst_pos = 0;
     for (int i = 0; i < DST_RING; i++) c->dst_copied[i] = nullptr;
+    c->rs_L = 0; c->rs_M = 0; c->d_G = nullptr; c->d_rcarry = nullptr; c->rs_k = 0; c->rs_b = 0; c->rs_p = 0;
     // driver entry point for the tensor-map encoder (no link-time dependency on libcuda)
     {
         void *fn = nullptr;
@@ -745,11 +989,14 @@ static int create(const Plan &pl, nrsc5b_channelizer_t **out, int device, const 
     }
     // the streaming staging buffer (cu8) or the cs16 byte planes as a [rows][64 B] capture matrix (rows past a launch's
     // valid bytes only feed outputs the launch does not write)
-    const size_t stage_cap = cs16 ? STAGE_CAP_CS16 : stage_cap_cu8(pl.taps), planes = cs16 ? 4 * PLANE_SAMPLES : 0;
+    // (a rate stage: the raw input staging - STAGE_CAP_CS16 bytes in either format - and the planes it writes)
+    if (ok && rs) ok = attach_rate(c, *rs);
+    const bool pl16 = reads_planes(c);
+    const size_t stage_cap = pl16 ? STAGE_CAP_CS16 : stage_cap_cu8(pl.taps), planes = pl16 ? 4 * PLANE_SAMPLES : 0;
     ok = ok && cudaMalloc(&c->d_stage, stage_cap) == cudaSuccess && cudaMemset(c->d_stage, 0, stage_cap) == cudaSuccess &&
          cudaEventCreateWithFlags(&c->stage_done, cudaEventDisableTiming) == cudaSuccess;
-    if (ok && cs16) ok = cudaMalloc(&c->d_planes, planes) == cudaSuccess && cudaMemset(c->d_planes, 0, planes) == cudaSuccess;
-    if (ok) ok = encode_maps(c, c->map_stage, cs16 ? c->d_planes : c->d_stage, cs16 ? planes : stage_cap);
+    if (ok && pl16) ok = cudaMalloc(&c->d_planes, planes) == cudaSuccess && cudaMemset(c->d_planes, 0, planes) == cudaSuccess;
+    if (ok) ok = encode_maps(c, c->map_stage, pl16 ? c->d_planes : c->d_stage, pl16 ? planes : stage_cap);
     if (ok)
         ok = cudaFuncSetAttribute(kernel_of(c), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(kpass)) == cudaSuccess;
     if (!ok) {
@@ -793,6 +1040,27 @@ extern "C" int nrsc5b_chan_create_fm_cs16(nrsc5b_channelizer_t **out, int device
     return pl ? create(*pl, out, device, offsets_100khz, nch, true) : NRSC5B_EINVAL;
 }
 
+// A capture at any rate fs (integer Hz) -> the plan of (mode, decim) through the rate stage; fs == R: the plan itself
+static int create_rate(nrsc5b_channelizer_t **out, int device, int mode, int decim, uint32_t rate_hz, const int *offsets, int nch, bool cs16)
+{
+    RateStage rs;
+    if (!out || !offsets || nch <= 0 || nch > 4096 || !rate_stage(mode, decim, rate_hz, &rs) || !rate_offsets_ok(rs, offsets, nch))
+        return NRSC5B_EINVAL;
+    return create(*rs.plan, out, device, offsets, nch, cs16, rs.L == 1 ? nullptr : &rs);
+}
+
+extern "C" int nrsc5b_chan_create_rate(nrsc5b_channelizer_t **out, int device, int mode, int decim, uint32_t rate_hz, const int *offsets,
+                                       int nch)
+{
+    return create_rate(out, device, mode, decim, rate_hz, offsets, nch, false);
+}
+
+extern "C" int nrsc5b_chan_create_rate_cs16(nrsc5b_channelizer_t **out, int device, int mode, int decim, uint32_t rate_hz,
+                                            const int *offsets, int nch)
+{
+    return create_rate(out, device, mode, decim, rate_hz, offsets, nch, true);
+}
+
 extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
 {
     if (!c) return;
@@ -802,6 +1070,8 @@ extern "C" void nrsc5b_chan_destroy(nrsc5b_channelizer_t *c)
     cudaFree(c->d_phasor);
     cudaFree(c->d_stage);
     cudaFree(c->d_planes);
+    cudaFree(c->d_G);
+    cudaFree(c->d_rcarry);
     cudaFree(c->d_dst);
     if (c->h_dst) cudaFreeHost(c->h_dst);
     if (c->stage_done) cudaEventDestroy(c->stage_done);
@@ -830,6 +1100,19 @@ extern "C" long long nrsc5b_chan_outputs_fm(int decim, size_t nbytes)
 {
     const Plan *pl = fm_plan(decim);
     return pl ? outputs_of(*pl, (long long)(nbytes / 2)) : NRSC5B_EINVAL;
+}
+/* N_plan(K(T)) for T input samples at fs */
+extern "C" long long nrsc5b_chan_outputs_rate(int mode, int decim, uint32_t rate_hz, long long samples)
+{
+    RateStage rs;
+    if (!rate_stage(mode, decim, rate_hz, &rs) || samples < 0) return NRSC5B_EINVAL;
+    return outputs_of(*rs.plan, rs.L == 1 ? samples : resampled_of(rs.L, rs.M, samples));
+}
+
+// the handle's outputs per channel from the first T input samples
+static long long outputs_in(const nrsc5b_channelizer *c, long long samples)
+{
+    return outputs_of(*c->plan, c->rs_L ? resampled_of(c->rs_L, c->rs_M, samples) : samples);
 }
 
 template <bool CS16, int KPASS, int Q>
@@ -863,7 +1146,7 @@ static int launch(nrsc5b_channelizer *c, const CUtensorMap *maps, long long n0, 
     if (slots < 1) slots = 1;
     if (slots > p.tiles) slots = p.tiles;
     const unsigned grid = (unsigned)(slots * c->ngroups);
-    const bool cs = c->cs16;
+    const bool cs = reads_planes(c);
     if (c->plan->taps != PASS_TAPS) (cs ? launch_k<true, 2, 1> : launch_k<false, 2, 1>)(maps, c->map_w, p, grid, stream);
     else if (c->plan->decim == 16) (cs ? launch_k<true, 1, 2> : launch_k<false, 1, 2>)(maps, c->map_w, p, grid, stream);
     else if (c->plan->decim == 8) (cs ? launch_k<true, 1, 4> : launch_k<false, 1, 4>)(maps, c->map_w, p, grid, stream);
@@ -880,6 +1163,57 @@ static int split_launch(nrsc5b_channelizer *c, const int16_t *src, long long nsa
     k_split_cs16<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(src, nvalues, c->d_planes, c->d_planes + 2 * PLANE_SAMPLES);
     if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
     return launch(c, c->map_stage, n0, nout, out, dst, out_stride, stream);
+}
+
+// Streaming through a rate stage.  Two carries: the input samples from b_{K(T)} on (at most 63) stay at the front of
+// d_stage, and the resampled samples from D N(K(T)) on (fewer than the plan's taps) are kept, as their two plane bytes,
+// in d_rcarry.  The planes are shared with the one-shot entry points, which write them from row 0, so a piece puts the
+// carry back at the front of the planes before it resamples behind it, and takes the new carry out again after the
+// channel bank has run.  A piece is bounded by both buffers: the raw staging holds STAGE_CAP_CS16 bytes, and the
+// piece's K(T') - K(T) <= piece L / M + 1 new resampled samples must fit the planes after the carry.
+static int stream_in_rate(nrsc5b_channelizer *c, const void *src, size_t nsamples, int16_t *out, const long long *dst, size_t out_stride,
+                          cudaMemcpyKind kind, cudaStream_t stream)
+{
+    const Plan &pl = *c->plan;
+    const int D = pl.decim, L = c->rs_L, M = c->rs_M;
+    const size_t bps = c->cs16 ? 4 : 2, cap = STAGE_CAP_CS16 / bps;
+    long long written = 0;
+    for (size_t done = 0; done < nsamples;) {
+        const size_t icarry = (size_t)(c->pushed - c->rs_b);
+        const long long first = outputs_of(pl, c->rs_k), rcarry = c->rs_k - D * first;
+        const long long room = (PLANE_SAMPLES - rcarry - 1) * M / L;
+        size_t piece = nsamples - done < cap - icarry ? nsamples - done : cap - icarry;
+        if ((long long)piece > room) piece = (size_t)room;
+        if (cudaMemcpyAsync(c->d_stage + bps * icarry, reinterpret_cast<const uint8_t *>(src) + bps * done, bps * piece, kind, stream) !=
+            cudaSuccess)
+            return NRSC5B_ECUDA;
+        const long long t1 = c->pushed + (long long)piece, k1 = resampled_of(L, M, t1), nk = k1 - c->rs_k;
+        const long long held = rcarry + nk, nl = outputs_of(pl, held);   // (nk = 0: nothing new, the planes are not read)
+        if (nk > 0) {
+            for (int pn = 0; rcarry > 0 && pn < 2; pn++)       // the resampled carry back to the front of both planes
+                if (cudaMemcpyAsync(c->d_planes + pn * 2 * PLANE_SAMPLES, c->d_rcarry + pn * 2 * RS_CARRY, 2 * (size_t)rcarry,
+                                    cudaMemcpyDeviceToDevice, stream) != cudaSuccess)
+                    return NRSC5B_ECUDA;
+            int rc = launch_resample(!c->cs16, c->d_stage, (long long)(icarry + piece), 0, c->rs_p, L, M, nk, c->d_G, c->d_planes, rcarry, stream);
+            if (rc) return rc;
+            const long long q = c->rs_p + nk * M, b1 = c->rs_b + q / L;   // nk M < 2^39: bounded by the piece
+            k_move_carry<<<1, (unsigned)(RS_TAPS * bps / 2), 0, stream>>>(c->d_stage, bps * (size_t)(b1 - c->rs_b), (int)(bps * (t1 - b1)));
+            if (cudaGetLastError() != cudaSuccess) return NRSC5B_ECUDA;
+            c->rs_p = (int)(q % L);
+            c->rs_b = b1;
+            c->rs_k = k1;
+            if (nl > 0 && (rc = launch(c, c->map_stage, first, nl, out + 2 * written, dst, out_stride, stream))) return rc;
+            const long long keep = held - D * nl;                // the new resampled carry, out of the planes
+            for (int pn = 0; keep > 0 && pn < 2; pn++)
+                if (cudaMemcpyAsync(c->d_rcarry + pn * 2 * RS_CARRY, c->d_planes + pn * 2 * PLANE_SAMPLES + 2 * D * nl, 2 * (size_t)keep,
+                                    cudaMemcpyDeviceToDevice, stream) != cudaSuccess)
+                    return NRSC5B_ECUDA;
+        }
+        c->pushed = t1;
+        written += nl;
+        done += piece;
+    }
+    return NRSC5B_OK;
 }
 
 // The streaming core of nrsc5b_chan_push* and nrsc5b_chan_feed*: appends nsamples complex samples (cu8 or cs16, the
@@ -901,6 +1235,11 @@ static int stream_in(nrsc5b_channelizer *c, const void *src, size_t nsamples, in
     cudaGetLastError();
     const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;
+    if (c->rs_L) {
+        const int rc = stream_in_rate(c, src, nsamples, out, dst, out_stride, kind, stream);
+        if (rc) return rc;
+        return cudaEventRecord(c->stage_done, stream) == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+    }
     long long written = 0;
     for (size_t done = 0; done < nsamples;) {
         const long long first = outputs_of(pl, c->pushed);        // absolute index of staging row 0's output
@@ -929,13 +1268,15 @@ extern "C" int nrsc5b_chan_reset(nrsc5b_channelizer_t *c)
 {
     if (!c) return NRSC5B_EINVAL;
     c->pushed = 0;                                            // the carry is what lies beyond D N(T): nothing now
+    c->rs_k = c->rs_b = 0;                                    // (a rate stage's two carries likewise)
+    c->rs_p = 0;
     return NRSC5B_OK;
 }
 
 // nsamples complex samples of the handle's format at src (checked by the caller)
 static int push(nrsc5b_channelizer *c, const void *src, size_t nsamples, void *d_out, size_t out_stride, void *cuda_stream, long long *nout)
 {
-    const long long n = outputs_of(*c->plan, c->pushed + (long long)nsamples) - outputs_of(*c->plan, c->pushed);
+    const long long n = outputs_in(c, c->pushed + (long long)nsamples) - outputs_in(c, c->pushed);
     if (n > 0 && (!d_out || ((uintptr_t)d_out & 3) || (out_stride & 1) || (size_t)(2 * n) > out_stride)) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const int rc = stream_in(c, src, nsamples, reinterpret_cast<int16_t *>(d_out), nullptr, out_stride,
@@ -963,7 +1304,7 @@ extern "C" int nrsc5b_chan_push_cs16(nrsc5b_channelizer_t *c, const int16_t *cs1
 // nsamples complex samples of the handle's format at src (checked by the caller)
 static int feed(nrsc5b_channelizer *c, nrsc5b_engine_t *e, const int *streams, const void *src, size_t nsamples)
 {
-    const long long n = outputs_of(*c->plan, c->pushed + (long long)nsamples) - outputs_of(*c->plan, c->pushed);
+    const long long n = outputs_in(c, c->pushed + (long long)nsamples) - outputs_in(c, c->pushed);
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const size_t nch = (size_t)c->nch;
     if (!c->h_dst) {
@@ -1011,17 +1352,48 @@ extern "C" int nrsc5b_chan_feed_cs16(nrsc5b_channelizer_t *c, nrsc5b_engine_t *e
     return feed(c, e, streams, cs16, nvalues / 2);
 }
 
+// One-shot through a rate stage: the device capture at src (16-byte aligned, nin samples of the handle's format) ->
+// out[nch][out_stride], PIECE_OUT plan outputs at a time: their resampled samples D n0 .. D (n0 + nl - 1) + taps - 1
+// (all below K(nin)) go from the caller's capture into the planes, and the plan runs on them.
+// (bank = false: the rate stage alone, the same launches of k_resample into the planes without the channel bank)
+static int run_rate(nrsc5b_channelizer *c, const void *src, long long nin, int16_t *out, size_t out_stride, cudaStream_t stream,
+                    bool bank = true)
+{
+    const int TAPS = c->plan->taps, D = c->plan->decim, L = c->rs_L, M = c->rs_M;
+    const long long PIECE_OUT = piece_out(TAPS, D);
+    const long long nout = outputs_in(c, nin);
+    if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;   // the planes are shared with the stream
+    for (long long n0 = 0; n0 < nout; n0 += PIECE_OUT) {
+        const long long nl = nout - n0 < PIECE_OUT ? nout - n0 : PIECE_OUT, r0 = D * n0, q = r0 * M;
+        int rc = launch_resample(!c->cs16, src, nin, q / L, (int)(q % L), L, M, D * nl + TAPS - D, c->d_G, c->d_planes, 0, stream);
+        if (!rc && bank) rc = launch(c, c->map_stage, n0, nl, out + 2 * n0, nullptr, out_stride, stream);
+        if (rc) return rc;
+    }
+    return cudaEventRecord(c->stage_done, stream) == cudaSuccess ? NRSC5B_OK : NRSC5B_ECUDA;
+}
+
+/* The rate stage of a rate handle's one-shot device path on its own (for timing it apart from the channel bank): the
+ * same k_resample launches into the handle's planes as nrsc5b_chan_run_device* makes for this capture (nvalues cu8
+ * bytes or cs16 int16 values, the handle's format, 16-byte aligned), and nothing else.  Asynchronous on cuda_stream. */
+extern "C" int nrsc5b_chan_resample_device(nrsc5b_channelizer_t *c, const void *d_in, size_t nvalues, void *cuda_stream)
+{
+    if (!c || !c->rs_L || !d_in || ((uintptr_t)d_in & 15) || (nvalues & 1)) return NRSC5B_EINVAL;
+    if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
+    return run_rate(c, d_in, (long long)(nvalues / 2), nullptr, 0, reinterpret_cast<cudaStream_t>(cuda_stream), false);
+}
+
 /* Device-resident capture (cu8, I/Q interleaved, 23 814 000 S/s; 64-byte aligned, nbytes of it valid) -> out[nch][out_stride]
  * cs16 on the device (out_stride in int16 values, >= 2 * outputs; 4-byte aligned rows).  Asynchronous on `cuda_stream`. */
 extern "C" int nrsc5b_chan_run_device(nrsc5b_channelizer_t *c, const void *d_cu8, size_t nbytes, void *d_out, size_t out_stride,
                                       void *cuda_stream)
 {
-    if (!c || c->cs16 || !d_cu8 || !d_out || ((uintptr_t)d_cu8 & 63) || (nbytes & 63) || ((uintptr_t)d_out & 3) || (out_stride & 1))
-        return NRSC5B_EINVAL;
-    const long long nout = outputs_of(*c->plan, (long long)(nbytes / 2));
+    if (!c || c->cs16 || !d_cu8 || !d_out || ((uintptr_t)d_out & 3) || (out_stride & 1)) return NRSC5B_EINVAL;
+    if (c->rs_L ? ((uintptr_t)d_cu8 & 15) || (nbytes & 1) : ((uintptr_t)d_cu8 & 63) || (nbytes & 63)) return NRSC5B_EINVAL;
+    const long long nout = outputs_in(c, (long long)(nbytes / 2));
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
+    if (c->rs_L) return run_rate(c, d_cu8, (long long)(nbytes / 2), reinterpret_cast<int16_t *>(d_out), out_stride, reinterpret_cast<cudaStream_t>(cuda_stream));
     // the capture as a [rows][64 B] matrix, one map per phase; rows past the end read as zero (only rows of outputs >= nout touch them)
     CUtensorMap map_x[4];
     if (!encode_maps(c, map_x, d_cu8, nbytes)) return NRSC5B_ECUDA;
@@ -1037,11 +1409,12 @@ extern "C" int nrsc5b_chan_run_device_cs16(nrsc5b_channelizer_t *c, const void *
         return NRSC5B_EINVAL;
     const int TAPS = c->plan->taps, D = c->plan->decim;
     const long long PIECE_OUT = piece_out(TAPS, D);
-    const long long nout = outputs_of(*c->plan, (long long)(nvalues / 2));
+    const long long nout = outputs_in(c, (long long)(nvalues / 2));
     if (nout <= 0) return NRSC5B_OK;
     if ((size_t)(2 * nout) > out_stride) return NRSC5B_EINVAL;
     if (cudaSetDevice(c->device) != cudaSuccess) return NRSC5B_ENODEV;
     const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (c->rs_L) return run_rate(c, d_cs16, (long long)(nvalues / 2), reinterpret_cast<int16_t *>(d_out), out_stride, stream);
     const int16_t *src = reinterpret_cast<const int16_t *>(d_cs16);
     int16_t *out = reinterpret_cast<int16_t *>(d_out);
     if (cudaStreamWaitEvent(stream, c->stage_done, 0) != cudaSuccess) return NRSC5B_ECUDA;   // the planes are shared with the stream
@@ -1079,9 +1452,9 @@ static int run_host(nrsc5b_channelizer *c, const void *in, size_t bytes, size_t 
 /* Host convenience (tests): host capture in, host cs16 out[nch][2 * outputs]. */
 extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, int16_t *out)
 {
-    if (!c || c->cs16 || !cu8 || !out) return NRSC5B_EINVAL;
-    nbytes &= ~(size_t)63;                                  // whole 64-byte rows (32 complex samples)
-    const long long nout = outputs_of(*c->plan, (long long)(nbytes / 2));
+    if (!c || c->cs16 || !cu8 || !out || (c->rs_L && (nbytes & 1))) return NRSC5B_EINVAL;
+    if (!c->rs_L) nbytes &= ~(size_t)63;                    // whole 64-byte rows (32 complex samples); a rate stage takes every sample
+    const long long nout = outputs_in(c, (long long)(nbytes / 2));
     if (nout <= 0) return NRSC5B_OK;
     return run_host(c, cu8, nbytes, nbytes, nout, out);
 }
@@ -1089,7 +1462,41 @@ extern "C" int nrsc5b_chan_run(nrsc5b_channelizer_t *c, const uint8_t *cu8, size
 extern "C" int nrsc5b_chan_run_cs16(nrsc5b_channelizer_t *c, const int16_t *cs16, size_t nvalues, int16_t *out)
 {
     if (!c || !c->cs16 || !cs16 || !out || (nvalues & 1)) return NRSC5B_EINVAL;
-    const long long nout = outputs_of(*c->plan, (long long)(nvalues / 2));
+    const long long nout = outputs_in(c, (long long)(nvalues / 2));
     if (nout <= 0) return NRSC5B_OK;
     return run_host(c, cs16, 2 * nvalues, nvalues, nout, out);
+}
+
+/* The rate stage alone, for kernel-level parity: host capture (cu8 bytes or cs16 int16 values, nvalues of them, even)
+ * at fs -> host out[2 K(T)] = y[0 .. K(T) - 1] (I, Q interleaved); synchronous.  fs == R has no stage: NRSC5B_EINVAL. */
+extern "C" int nrsc5b_resample(int device, int mode, int decim, uint32_t rate_hz, int cs16, const void *in, size_t nvalues, int16_t *out)
+{
+    RateStage rs;
+    if (!rate_stage(mode, decim, rate_hz, &rs) || rs.L == 1 || (nvalues & 1) || (nvalues && (!in || !out))) return NRSC5B_EINVAL;
+    const long long T = (long long)(nvalues / 2), K = resampled_of(rs.L, rs.M, T);
+    if (K <= 0) return NRSC5B_OK;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device >= ndev || cudaSetDevice(device) != cudaSuccess) return NRSC5B_ENODEV;
+    std::vector<int16_t> G;
+    design_resampler(rs, G);
+    const size_t bytes = nvalues * (cs16 ? 2 : 1);
+    const long long PIECE = 1ll << 22;
+    uint8_t *d_in = nullptr, *d_planes = nullptr;
+    int16_t *d_G = nullptr;
+    std::vector<uint8_t> hi(2 * (size_t)PIECE), lo(2 * (size_t)PIECE);
+    bool ok = cudaMalloc(&d_in, (bytes + 15) & ~(size_t)15) == cudaSuccess && cudaMalloc(&d_planes, 4 * PLANE_SAMPLES) == cudaSuccess &&
+              cudaMalloc(&d_G, G.size() * sizeof(int16_t)) == cudaSuccess && cudaMemcpy(d_in, in, bytes, cudaMemcpyHostToDevice) == cudaSuccess &&
+              cudaMemcpy(d_G, G.data(), G.size() * sizeof(int16_t), cudaMemcpyHostToDevice) == cudaSuccess;
+    for (long long r0 = 0; ok && r0 < K; r0 += PIECE) {
+        const long long nr = K - r0 < PIECE ? K - r0 : PIECE, q = r0 * rs.M;
+        ok = launch_resample(!cs16, d_in, T, q / rs.L, (int)(q % rs.L), rs.L, rs.M, nr, d_G, d_planes, 0, nullptr) == NRSC5B_OK &&
+             cudaMemcpy(hi.data(), d_planes, 2 * nr, cudaMemcpyDeviceToHost) == cudaSuccess &&
+             cudaMemcpy(lo.data(), d_planes + 2 * PLANE_SAMPLES, 2 * nr, cudaMemcpyDeviceToHost) == cudaSuccess;
+        for (long long v = 0; ok && v < 2 * nr; v++) out[2 * r0 + v] = (int16_t)(256 * (int8_t)hi[v] + lo[v]);
+    }
+    if (!ok) fprintf(stderr, "nrsc5_b200: resampler failed: %s\n", cudaGetErrorString(cudaGetLastError()));
+    cudaFree(d_in);
+    cudaFree(d_planes);
+    cudaFree(d_G);
+    return ok ? NRSC5B_OK : NRSC5B_ECUDA;
 }
