@@ -438,6 +438,120 @@ int nrsc5b_resample(int device, int mode, int decim, uint32_t rate_hz, int cs16,
  * 16-byte aligned), into the handle's own scratch; no channel output.  NRSC5B_EINVAL on a handle without a stage. */
 int nrsc5b_chan_resample_device(nrsc5b_channelizer_t *c, const void *d_in, size_t nvalues, void *cuda_stream);
 
+/* ---- band scan: which channels carry an NRSC-5 signal (the reference has no counterpart; the nearest thing is the
+ * coarse acquisition of one stream, reference src/acquire.c:120-158: band-pass, fold the cyclic-prefix correlation
+ * over 32 symbols, take the arg-max) ----
+ * Input: channel output y[n], complex int16, what nrsc5b_chan_* writes: FM channels at 744 187.5 S/s, AM channels at
+ * 46 511.71875 S/s.  Per mode, lag F (the FFT length), CP length P, symbol S = F + P, subsampling q and the sidebands:
+ *     FM: F = 2048, P = 112, S = 2160, q = 4; carriers -478..-356 / +356..+478 (129.4 - 173.7 kHz), in the primary
+ *         main partitions every FM service mode has.  Not the whole partition (up to carrier 546, 198.4 kHz): a station
+ *         400 kHz away has its own sideband from 202 kHz on, and 64 taps need about 28 kHz for 40 dB, so the band stops
+ *         short of it as it stops short of the channel's own analogue host (100 kHz)
+ *     AM: F = 256,  P = 14,  S = 270,  q = 2; carriers -81..-33 / +33..+81 (6.0 - 14.7 kHz).  The inner carriers
+ *         2..32 lie under a hybrid (MA1) station's analogue audio, far stronger than they are, and in an all-digital
+ *         (MA3) station their lag-F correlation comes out with the wrong sign (measured -0.50 per unit energy over
+ *         0.36 - 5 kHz against +0.58 and +0.66 over 5 - 10 and 10 - 15 kHz), which would put the CFO half a
+ *         subcarrier off
+ * With g_U[u], u < 64, the upper sideband's Q15 taps (nrsc5b_scan_make_tables) and g_L = conj(g_U), for s in {L, U}:
+ *     z_s[n]    = sat16((sum_u g_s[u] y[n - 63 + u] + 2^14) >> 15)      per component, n = 0 (mod q), n >= 63
+ *     p_s[n]    = z_s[n] conj(z_s[n + F]),   e_s[n] = |z_s[n]|^2 + |z_s[n + F]|^2          exact in int64
+ *     Fold_s[j] = sum_m p_s[q j + m S],      En_s[j] likewise                                j < J = S / q
+ *     C_s[j]    = sum_{i < P/q} Fold_s[(j + i) mod J],   E_s[j] likewise over En_s
+ * n counts from the first sample the scan was given; a product counts once both its samples have been (n + F < T, T
+ * the samples pushed since create / reset).  |Re p|, |Im p| <= 2^31 and e <= 2^32, so Fold and En fit int64 up to 2^24
+ * symbols: a push that takes T / S beyond 2^24 returns NRSC5B_EINVAL and changes nothing.
+ * Taps: a Kaiser-windowed sinc low-pass moved to the sideband, unit passband gain (Q15: 32768), sum |Re g| and
+ * sum |Im g| below 2^16.  FM: centred on 151 kHz, -6 dB 37 kHz either side, >= 40 dB down at |f| <= 100 kHz (the
+ * channel's own analogue host) and at f >= 202 kHz (the sideband of a station 400 kHz away; measured 41.3 dB both),
+ * within 0.5 dB over carriers 356..478 (measured 0.13 dB).  AM: centred on
+ * 10.4 kHz, -6 dB 5 kHz either side, with the window subtracted in proportion so that sum g = 0 exactly: an exact null
+ * at DC (the analogue carrier), flat within 0.5 dB over 6.5 - 14 kHz (measured 0.11 dB; 64 taps at 46.5 kS/s cannot
+ * resolve a sharper edge) and 15.6 dB down at 5 kHz.
+ * Metrics (nrsc5b_scan_result; in double, ties to the smallest j; phi = q j):
+ *     C = C_L + C_U, mean C' = sum_j C[j] / J, j* = argmax_j |C[j] - C'|: the mean removes every stationary component
+ *         in expectation (tones, spurs, an analogue host, a neighbour's host inside the sideband); a CP-periodic (OFDM)
+ *         signal survives
+ *     score     = |C[j*] - C'| / (1/2 (E_L + E_U)[j*])
+ *     symbols   M = N_p q / S, N_p the products counted per sideband
+ *     score_s   = |C_s[j*] - C'_s| / (1/2 E_s[j*]), each sideband at the timing found
+ *     threshold tau(M) = c / sqrt(M P / q),  threshold_sideband tau_1(M) = c1 / sqrt(M P / q)
+ *     detected  = M >= 32 and score >= tau(M) and score_L >= tau_1(M) and score_U >= tau_1(M) and
+ *               Re(D_L conj(D_U)) >= cos(45 deg) |D_L| |D_U|, D_s = C_s[j*] - C'_s
+ *               Both sidebands must carry the CP correlation: a station's one sideband also falls into the filter
+ *               of the channel 300 kHz (FM; AM: 20 kHz) beside it - its upper sideband, +129..+198 kHz, is the lower
+ *               passband, -174..-129 kHz, of the channel 300 kHz above - where the combined score alone reaches
+ *               almost the station's own; there the other sideband holds no correlation at that timing.  And both
+ *               must agree in phase: the two sidebands of one station share its carrier, so their correlations share
+ *               its CFO, while an AM channel 10 kHz beside a station takes the station's inner carriers into one
+ *               filter and its spectrum beyond 15 kHz into the other (measured 53 - 63 degrees apart on synthetic MA1
+ *               and MA3 stations 60 dB over the noise, against at most 11 degrees in the stations' own channels).
+ *               What still holds: (1) a channel whose two sidebands take one sideband each of two stations with the
+ *               same symbol timing (to within the window) and CFO would pass; independent stations share neither on
+ *               purpose, so this needs two transmitters locked to each other 600 kHz (AM: 40 kHz) apart.  (2) The
+ *               stopbands are about 40 dB: a station some 45 dB or more over the noise leaks into both filters of the
+ *               channels 100 kHz (AM: 10 - 20 kHz) beside it, with its own timing and phase, and can be detected
+ *               there too; its score there stays far below the station's own.
+ *     timing    = (q j* - 32) mod S: the first CP sample of a symbol in the channel's own sample index (the taps' group
+ *               delay of 31.5 samples removed)
+ *     cfo_hz    = -arg(C[j*] - C') fs / (2 pi F): the CFO within +-1/2 subcarrier, in the channel's own spectrum
+ *     rho_s     = |C_s[j*] - C'_s| / (1/2 mean_j E_s[j]);  snr_db_s = 10 log10(rho_s / (kappa - rho_s)), -inf / +inf
+ *               outside (0, kappa).  The energy averaged over all timings, not E_s[j*]: the pulse shape (reference
+ *               src/acquire.c:320-342) halves the signal's energy at the CP while the noise stays uniform.
+ *     power_dbfs = 10 log10(mean |y|^2 / 2^30) over the samples given; power_dbfs_lower / _upper likewise of z_s over
+ *               the products' samples (sum_j En_s[j] / 2 N_p)
+ * c: under noise alone, z_s is complex Gaussian and C - C' a sum of N = M P / q products, so score = R sqrt(gamma / 2N)
+ * with R^2 ~ Exp(1) and gamma = sum_k |r(k q)|^2 the products' correlation (r: the normalised autocorrelation of g_U;
+ * 2.542 FM, 2.342 AM).  Treating the J positions as independent (neighbours are correlated, so this errs on the safe
+ * side), P(max R > r) = J e^(-r^2) = 1e-6 per channel gives r^2 = ln(1e6 J) and c = sqrt(gamma ln(1e6 J) / 2).
+ * c1: for one sideband at a given timing (not a maximum over J), score_s = R sqrt(gamma / N), and P(R > r) = e^(-r^2)
+ * = 1e-3 gives c1 = sqrt(gamma ln(1e3)): with the 1e-6 of tau(M) in front of it, a sideband that holds only noise
+ * passes tau_1 once in a thousand, while a station at -3 dB per sideband passes it in half a second.
+ * kappa: the mean of rho_L and rho_U for a noise-free synthetic station (the pulse shape's 1/pi, less the filter's
+ * spread), measured with the numpy restatement (tests/scan_oracle.py) on one MP1 frame (1.49 s, decimated from the
+ * generator's 1 488 375 S/s; FM: 0.3163 and 0.3042) and four MA3 frames (AM: 0.3145 and 0.3107). */
+#define NRSC5B_SCAN_C_FM 5.055
+#define NRSC5B_SCAN_C_AM 4.682
+#define NRSC5B_SCAN_C1_FM 4.190
+#define NRSC5B_SCAN_C1_AM 4.022
+#define NRSC5B_SCAN_KAPPA_FM 0.310
+#define NRSC5B_SCAN_KAPPA_AM 0.313
+/* raw int64 values per channel of nrsc5b_scan_result: Fold_L re, im, En_L, Fold_U re, im, En_U, then C_L re, im, E_L,
+ * C_U re, im, E_U, each [J]; then sum |y|^2 as two uint64 words (low, high).  J = 540 (FM), 135 (AM). */
+#define NRSC5B_SCAN_RAW(J) (12 * (J) + 2)
+typedef struct {
+    double score, threshold, symbols, cfo_hz;
+    double score_lower, score_upper, threshold_sideband;
+    double snr_db_lower, snr_db_upper;
+    double power_dbfs, power_dbfs_lower, power_dbfs_upper;
+    int32_t detected;
+    int32_t timing;
+} nrsc5b_scan_t;
+typedef struct nrsc5b_scanner nrsc5b_scanner_t;
+/* A scanner of `nch` channels of mode NRSC5B_MODE_FM or NRSC5B_MODE_AM; NRSC5B_ENODEV without a device. */
+int nrsc5b_scan_create(nrsc5b_scanner_t **out, int device, int mode, int nch);
+void nrsc5b_scan_destroy(nrsc5b_scanner_t *s);
+/* Start over: T = 0, every accumulator 0. */
+int nrsc5b_scan_reset(nrsc5b_scanner_t *s);
+/* The next nsamples of every channel: device memory [nch][stride] int16 values (4-byte aligned, stride even and
+ * >= 2 nsamples), asynchronous on cuda_stream (a cudaStream_t cast to void*, NULL = default).  The handle keeps the
+ * last F + 63 samples of every channel, so a capture pushed in pieces of any size gives every accumulator of the
+ * one-shot scan bit for bit. */
+int nrsc5b_scan_push_device(nrsc5b_scanner_t *s, const void *d_ch, size_t stride, size_t nsamples, void *cuda_stream);
+/* The same from host memory [nch][2 nsamples]; synchronous (tests). */
+int nrsc5b_scan_push(nrsc5b_scanner_t *s, const int16_t *cs16, size_t nsamples);
+/* The metrics of every channel so far (out[nch]); raw (optional): [nch][NRSC5B_SCAN_RAW(J)] the exact sums.  Waits for
+ * the pushes; the scan goes on from where it is. */
+int nrsc5b_scan_result(nrsc5b_scanner_t *s, nrsc5b_scan_t *out, int64_t *raw);
+/* Channelise and scan: the capture (nvalues cu8 bytes or cs16 values, the handle's format, host or device memory) goes
+ * through the channeliser's streaming push (nrsc5b_chan_push*: every plan, decim and rate handle) into the scanner's
+ * own device buffer and from there into the scan, piece by piece, on the default CUDA stream; no channel output comes
+ * back to the host.  The scanner must have the plan's mode, device and channel count (channel k = the plan's channel
+ * k); otherwise, for odd nvalues, or if the scan would pass 2^24 symbols: NRSC5B_EINVAL, neither handle changed.  The
+ * scanner's buffer is 2^18 bytes per channel, allocated at the first call. */
+int nrsc5b_chan_scan(nrsc5b_channelizer_t *c, nrsc5b_scanner_t *s, const void *capture, size_t nvalues);
+/* The upper sideband's taps[64][2] (Re, Im of g_U; g_L = conj(g_U)) and kappa for the mode, without a device. */
+int nrsc5b_scan_make_tables(int mode, int16_t *taps, double *kappa);
+
 const char *nrsc5b_version(void);
 
 #ifdef __cplusplus

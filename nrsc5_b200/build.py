@@ -20,6 +20,7 @@ UNITS = [
     ("frontend.cu", []),
     ("engine.cu", ["-fmad=false"]),
     ("channelizer.cu", []),
+    ("scan.cu", []),
 ]
 
 

@@ -92,6 +92,7 @@
 
 #include "../../include/nrsc5_b200.h"
 #include "chan_feed.h"
+#include "chan_scan.h"
 
 namespace nbch {
 
@@ -1283,6 +1284,21 @@ static int push(nrsc5b_channelizer *c, const void *src, size_t nsamples, void *d
                              reinterpret_cast<cudaStream_t>(cuda_stream));
     if (rc == NRSC5B_OK && nout) *nout = n;
     return rc;
+}
+
+int nbchan_info(const nrsc5b_channelizer_t *c, int *device, int *mode, int *cs16, int *nch)
+{
+    if (!c) return NRSC5B_EINVAL;
+    *device = c->device;
+    *mode = c->plan->engine_mode;
+    *cs16 = c->cs16;
+    *nch = c->nch;
+    return NRSC5B_OK;
+}
+
+long long nbchan_outputs_after(const nrsc5b_channelizer_t *c, long long samples)
+{
+    return outputs_in(c, c->pushed + samples) - outputs_in(c, c->pushed);
 }
 
 extern "C" int nrsc5b_chan_push(nrsc5b_channelizer_t *c, const uint8_t *cu8, size_t nbytes, void *d_out, size_t out_stride,
