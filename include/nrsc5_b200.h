@@ -552,6 +552,103 @@ int nrsc5b_chan_scan(nrsc5b_channelizer_t *c, nrsc5b_scanner_t *s, const void *c
 /* The upper sideband's taps[64][2] (Re, Im of g_U; g_L = conj(g_U)) and kappa for the mode, without a device. */
 int nrsc5b_scan_make_tables(int mode, int16_t *taps, double *kappa);
 
+/* ---- band receiver: every HD Radio station of a live wideband capture decoded, engines attached and detached as the
+ * scan finds and loses stations (the reference has no counterpart: it takes one narrowband device per handle,
+ * reference src/nrsc5.c:130-207) ----
+ * One handle owns a channeliser of the plan (nrsc5b_chan_create_fm / _am / _rate, cu8 or cs16), a scanner of its
+ * channels and one cs16 engine of the plan's mode with max_stations streams (nrsc5b_enable_l2 if l2 != 0).
+ * Pipeline, per push of any size:
+ *   1. Every channel is channelised once (nrsc5b_chan_push*) into a device window buffer of W = window_symbols x S
+ *      samples per channel (S = 2160 FM, 270 AM).  The capture is split so that windows fill exactly (a rate stage's
+ *      one input sample can emit several outputs; those past W open the next window).  Channel sample n counts the
+ *      plan's outputs from the first sample pushed; window w holds n in [wW, (w+1)W).
+ *   2. A full window gets a verdict: nrsc5b_scan_push_device of its W samples, nrsc5b_scan_result, nrsc5b_scan_reset.
+ *      Window w's rows are exactly the one-shot scan of channel samples [wW, (w+1)W); the scan's 2^24-symbol bound
+ *      never applies (a window is at most 512 symbols).
+ *   3. The policy, on the host, once per window, in this order:
+ *      Suppression.  A detected channel k is leakage if some other detected channel j has |m_j - m_k| <= r (r = 1 FM,
+ *        2 AM, in grid steps), a higher score (equal scores: the smaller m wins) and a timing within P / 2 samples
+ *        mod S (56 FM, 7 AM; P the cyclic prefix).  A station some 45 dB or more over the noise is detected in the
+ *        channels beside it too, with its own timing (case (2) of the scan's "What still holds"); this takes those out.
+ *        The timing found there wanders with the leaked content: on synthetic FM stations 60 dB over the noise it came
+ *        out more than the scan's 2q (8 samples) off the station's own, and a tolerance of 2q opened a second session
+ *        on the neighbour.  P / 2 is the top half of the CP window sum's triangle around the station's timing.
+ *        Present = detected and not leakage.  Not covered: an AM channel 10 kHz beside an MA1 station scores above the station itself (about 1.2
+ *        against 0.6 on a synthetic MA1 station) and is normally refused by the scan's phase rule; in a
+ *        window where it passes, this rule keeps the neighbour and flags the station as leakage.
+ *      Detach.  A session whose channel has not been present in hold_windows consecutive windows closes: n1 = the end
+ *        of its last routed window (wW in window w), the engine runs, its records are drained into the session, the
+ *        stream is reset (nrsc5b_reset) and freed.  A channel present again later opens a new session.
+ *      Attach.  A present channel without a session gets the lowest free engine stream; its session starts at the
+ *        start of this window, n0 = wW: the window is kept until its verdict, so no sample of it is lost.  No stream
+ *        free: the channel's row is flagged NRSC5B_BAND_NO_SLOT.  Channels are taken in index order.
+ *   4. Route: k_band_route appends the window's samples of every open session's channel to its engine stream, on the
+ *      engine's CUDA stream, one launch per window; no channel data passes through the host.  A stream without room
+ *      (its 4 MiB input buffer; a 512-symbol FM window is 4.4 MB) makes the engine run, and the route goes on in
+ *      pieces: no sample is dropped.
+ *   5. nrsc5b_process, then every open session's records are drained into a host buffer of its own.  A stream's record
+ *      log (2 MiB) holds what one window's processing can emit; should it ever overflow, the push fails with
+ *      NRSC5B_EOVERFLOW instead of truncating.
+ * So a session's records are those of a cs16 engine of the same mode (and L2 setting) given channel samples
+ * [n0, n1) by nrsc5b_push_cs16 and processed, except the positions in REC_BLOCK, which count from where the stream's
+ * input buffer was last trimmed.  REC_L2's frame_off counts from the start of each nrsc5b_band_records output. */
+typedef struct nrsc5b_band nrsc5b_band_t;
+typedef struct {
+    int device, mode, decim;        /* NRSC5B_MODE_FM: decim 8 | 16 | 32; NRSC5B_MODE_AM: 32 */
+    uint32_t rate_hz;               /* 0: the plan's own rate, else the rate stage (nrsc5b_chan_create_rate*) */
+    int input_cs16;
+    const int *offsets; int nch;    /* NULL (nch = 0): every grid point the plan (and rate) takes, -lim ..= lim with lim =
+                                     * 117 / 59 / 29 (FM, D = 32 / 16 / 8) or 74 (AM), or the rate stage's largest usable
+                                     * |offset| where it is smaller.  Otherwise distinct offsets within that range */
+    int window_symbols;             /* 32 ..= 512 */
+    int hold_windows;               /* >= 1 */
+    int max_stations;               /* engine streams, 1 ..= 4096 */
+    int l2;
+} nrsc5b_band_config_t;
+enum {
+    NRSC5B_BAND_DETECTED = 1,       /* the scan's verdict */
+    NRSC5B_BAND_LEAKAGE = 2,        /* detected, but a stronger neighbour's leakage (not present) */
+    NRSC5B_BAND_ATTACHED = 4,       /* a session holds the channel after this window's policy: the window is routed to it */
+    NRSC5B_BAND_NO_SLOT = 8,        /* present without a session, and no engine stream was free */
+};
+typedef struct {
+    int32_t id;                     /* 0, 1, ... in the order sessions open */
+    int32_t channel, offset;        /* channel index and its offset (grid steps) */
+    int32_t slot;                   /* engine stream; -1 once closed */
+    int64_t n0, n1;                 /* channel samples [n0, n1) went to the engine; n1 = -1 while open */
+    int64_t window;                 /* the window whose verdict opened it (n0 = window x W) */
+    nrsc5b_scan_t verdict;          /* that window's row of the channel */
+} nrsc5b_band_session_t;
+/* EINVAL for a bad config (checked first, without a device), ENODEV without a device. */
+int nrsc5b_band_create(nrsc5b_band_t **out, const nrsc5b_band_config_t *cfg);
+void nrsc5b_band_destroy(nrsc5b_band_t *b);
+/* The next nvalues of the capture: cu8 bytes or cs16 int16 values (the config's format), host or device memory, even.
+ * Synchronous: returns once the capture has been read (the buffer may be reused at once, page-locked and device memory
+ * included) and every window it completes has been scanned, routed and processed.  Odd nvalues, or a push after
+ * nrsc5b_band_flush: NRSC5B_EINVAL, nothing changed. */
+int nrsc5b_band_push(nrsc5b_band_t *b, const void *capture, size_t nvalues);
+/* End of the capture: the partial window is routed (it gets no verdict), the engine runs and every session closes at
+ * n1 = the last channel sample.  Later pushes are refused; a second flush does nothing. */
+int nrsc5b_band_flush(nrsc5b_band_t *b);
+/* Takes up to cap completed windows, oldest first: index[i], rows[i][nch], flags[i][nch] (NRSC5B_BAND_*; any pointer
+ * may be NULL).  Returns the number taken; *pending (may be NULL) = windows waiting before the call.  Windows wait here
+ * until taken (about 100 bytes per channel each: some 0.2 GB an hour for 235 FM channels at 128 symbols), so a
+ * long-running caller takes them; one that does not want them discards them with index, rows and flags NULL and cap
+ * at least the pending count. */
+int nrsc5b_band_windows(nrsc5b_band_t *b, int64_t *index, nrsc5b_scan_t *rows, uint32_t *flags, int cap, int *pending);
+/* Every session opened so far, by id (not drained): writes min(cap, *n) and returns that number. */
+int nrsc5b_band_sessions(nrsc5b_band_t *b, nrsc5b_band_session_t *out, int cap, int *n);
+/* Session id's records since the last call, in the engine's record format; as nrsc5b_drain: returns the bytes
+ * written, *needed = the bytes waiting, NRSC5B_EFULL (nothing taken) if cap is smaller.  A closed session's buffer is
+ * freed once taken. */
+long nrsc5b_band_records(nrsc5b_band_t *b, int id, uint8_t *out, size_t cap, size_t *needed);
+/* The channel offsets (offsets[nch], may be NULL) and their number. */
+int nrsc5b_band_channels(nrsc5b_band_t *b, int *offsets, int *nch);
+/* Device time per stage since create, from CUDA events on the handle's work: ms4 = {channelise (nrsc5b_chan_push*),
+ * scan (push, result, reset: readback included), route (k_band_route), engine (nrsc5b_process)}; route_bytes = bytes
+ * k_band_route read and wrote. */
+int nrsc5b_band_times(nrsc5b_band_t *b, double *ms4, unsigned long long *route_bytes);
+
 const char *nrsc5b_version(void);
 
 #ifdef __cplusplus

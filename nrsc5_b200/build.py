@@ -21,6 +21,7 @@ UNITS = [
     ("engine.cu", ["-fmad=false"]),
     ("channelizer.cu", []),
     ("scan.cu", []),
+    ("band.cu", []),
 ]
 
 
