@@ -255,7 +255,9 @@ __global__ void __launch_bounds__(V64_FWD_THREADS) k_v64_fwd(V64Args a)
     // saturation guard (see viterbi_chunk.cuh): between two of the reference's normalisations (every 79
     // steps) the metrics grow by at most the sum of |s0|+|s1|+|s2|; with a spread of at most 12*381 after
     // a normalisation, sums <= 32767 - 12*381 cannot saturate.  Every 79-step window lies inside the
-    // range (warm-up included) of at least one chunk.
+    // range (warm-up included) of at least one chunk, which compares it when it reaches the window's
+    // closing normalisation; the frame's last window has none, so the chunk that ends the frame compares
+    // it after its last step.
     const int sat_limit = 32767 - 12 * 381;
     int wsum = 0;
     bool bad = false;
@@ -342,6 +344,7 @@ __global__ void __launch_bounds__(V64_FWD_THREADS) k_v64_fwd(V64Args a)
             for (int i = 0; i < 32; i++) o[i] = vs.P[i];
         }
     }
+    if (s_end == total) bad |= wsum > sat_limit;
     {
         uint32_t *o = a.vend + ((size_t)f * a.nch + c) * 32;
 #pragma unroll
